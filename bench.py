@@ -60,23 +60,11 @@ def load_peaks():
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return {"tflops": float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0))),
-                "tflops_burst": float(d.get("bf16_tflops", 1590.0)), "hbm_gbs": float(d.get("hbm_gbs", 6650.0)),
+        return {"tflops": float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 989.0))),
+                "tflops_burst": float(d.get("bf16_tflops", 989.0)), "hbm_gbs": float(d.get("hbm_gbs", 3350.0)),
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"tflops": 1400.0, "tflops_burst": 1590.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
-
-
-def load_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum of the dominant kernel, per launch, from the committed
-    `ncu --set full` capture of this same workload (profiles/r02_attn_traffic.json, else round 1's); None if absent."""
-    for name in ("r02_attn_traffic.json", "r01_attn_traffic.json"):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                d = json.load(f)
-            return {"bytes_per_launch": d["traffic_bytes_per_launch"], "unit": "B", "source": d["source"]}
-        except Exception:
-            continue
-    return None
+    # H100 SXM data sheet (700 W): dense fp16 / bf16 tensor rate and HBM3 bandwidth; a denominator, not a measurement
+    return {"tflops": 989.0, "tflops_burst": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
@@ -304,6 +292,7 @@ class Workload:
             out = self._forward(i, lat, prompt)
         if host_io:
             self.out_host.copy_(out, non_blocking=True)
+        self.last_out = out
         return out
 
 
@@ -538,6 +527,9 @@ def main():
                          "optimisation and GMFlow's correlation kernel; replicas: one independent N=8 batch per GPU")
     ap.add_argument("--graphs", default="auto", choices=["auto", "on", "off"],
                     help="replay the step from CUDA graphs (auto: on for the frame-sharded workload)")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write the UNet output of the last timed step as DIR/unet_out.npy "
+                         "(float32); the inputs depend only on the arguments, so two builds can be compared")
     ap.add_argument("--profile-mode", action="store_true",
                     help="for ncu captures only: 1 warm-up + --steps, no e2e / cpu baseline; never a bench value")
     args = ap.parse_args()
@@ -560,7 +552,7 @@ def main():
                           "warp_tensor fusion on 4 decoder features; 15-step DDPM schedule t=700..0 walked cyclically",
               "frames": N_FRAMES, "resolution": RES,
               "parallelism": "one GPU" if world == 1 else "replicas x%d (one 8-keyframe batch per GPU)" % world,
-              "l2": "working set (1.7 GB weights + activations) >> 126 MB L2, no explicit flush"}
+              "l2": "working set (1.7 GB weights + activations) >> 50 MB L2, no explicit flush"}
 
     if args.impl == "reference":
         config["parallelism"] = "host cores only (rank 0); n_gpus echoes --gpus"
@@ -636,6 +628,10 @@ def main():
     sampler.start()
     ms = timed_region(wl, args.steps, args.warmup, False, world)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "unet_out.npy"), wl.last_out.float().cpu().numpy())
     launches = _lib.launch_count() - launches0
     prof = ops.PROFILE
     ops.PROFILE = None
@@ -682,7 +678,7 @@ def main():
         roof = {"kernel": "%s (cross-frame, L=%d, Lk=%d, B=%d, 8 heads)" % (_lib.lib().fresco_attn_variant(40).decode(), L_b,
                                                                                 wl.kv_len[L_b], n_q),
                 "bound": "tensor", "achieved": kd["achieved"], "peak": peaks["tflops"], "unit": "TFLOP/s",
-                "frac": kd["frac"], "traffic": load_traffic(), "peak_source": peaks["source"],
+                "frac": kd["frac"], "peak_source": peaks["source"],
                 "algorithmic_flops_per_launch": kd["work"], "avg_launch_ms": kd["ms"], "launches_timed": kd["launches"],
                 "share_of_step_time": round(kd["total_ms"] / (prof_steps / float(args.steps) * ms), 4)
                 if wl.graphs is None else None,
@@ -720,7 +716,7 @@ def main():
         print(json.dumps(line), flush=True)
     if world > 1:
         # Leave without tearing NCCL down: destroying a process group whose collectives live in captured CUDA graphs
-        # hung for the full timeout on the 2-GPU box (profiles/README.md); everything is printed and flushed by now.
+        # can hang for the full timeout; everything is printed and flushed by now.
         import torch.distributed as dist
         dist.barrier()
         torch.cuda.synchronize()

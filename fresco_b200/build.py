@@ -1,9 +1,8 @@
-"""Build libfresco_b200.so (hand-written sm_100a kernels + C ABI) in-tree with nvcc.
+"""Build libfresco_b200.so (hand-written sm_90a kernels + C ABI) in-tree with nvcc.
 
     python -m fresco_b200.build [--force]
 
-nvcc cross-compiles without a GPU; the resulting .so is git-ignored but travels
-to the GPU box with the gpurun snapshot.
+nvcc cross-compiles without a GPU; the resulting .so and objects are git-ignored build products.
 """
 from __future__ import annotations
 
@@ -18,11 +17,11 @@ TAG = os.environ.get("FRESCO_BUILD_TAG", "")                 # A/B builds only: 
 OBJ = os.path.join(HERE, "csrc", "_obj" + TAG)
 LIB = os.path.join(HERE, "libfresco_b200%s.so" % TAG)
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--use_fast_math=false",
          "-Xptxas", "-v", "-I", os.path.join(os.path.dirname(HERE), "include")]
 FLAGS = [f for f in FLAGS if f != "--use_fast_math=false"]
-FLAGS += os.environ.get("FRESCO_NVCC_EXTRA", "").split()      # profiling builds only (-DFRESCO_ATTN_TRACE ...)
+FLAGS += os.environ.get("FRESCO_NVCC_EXTRA", "").split()      # extra nvcc flags for experimental builds
 
 
 def sources():

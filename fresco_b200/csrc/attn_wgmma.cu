@@ -1,0 +1,433 @@
+// FRESCO attention forward (spatial-guided and cross-frame SDPA) for sm_90a.
+//
+// Replaces the two dense F.scaled_dot_product_attention calls of the reference processor
+// (src/diffusion_hacked.py:281-285 and :303-305).
+//
+// TMA + wgmma flash attention.  Token-major [batch, tokens, heads*head_dim] fp16 tensors are consumed in place -- the TMA
+// tensor map views them as {head_dim, heads, tokens, batch}; a {64,1,rows,1} box lands one head's tile in the canonical
+// 128B-swizzled K-major layout; columns >= head_dim and rows >= tokens are hardware zero-filled (no padding passes for
+// head_dim 40 / 80 or ragged lengths).
+//
+//   last warp     TMA producer: Q once, K/V tiles of KN keys through an mbarrier ring of as many stages (<= 4) as fit
+//   NWG x 4 warps consumer warpgroups, 64 query rows each.  Per key tile: S = Q K^T by wgmma (A and B from shared
+//                 memory, fp32 accumulators in registers), online softmax in registers (a query row lives in the four
+//                 lanes of a quad), P converted to fp16 A fragments in registers, O += P V by wgmma with A from registers
+//                 and V read MN-major from the same swizzled tile.  The warpgroups drift apart, so the tensor core
+//                 works for one while the others are in their exponentials.
+//
+// Variants (fresco_set_option / environment, read once; every one is parity-tested at every head_dim):
+//   FRESCO_ATTN_WIDE    0: 64-key tiles, two consumer warpgroups; 1 (default): 128-key tiles, two warpgroups;
+//                       2: 128-key tiles, three warpgroups (192 query rows per CTA; head_dim <= 64, else as 1:
+//                       at 80 the 416-thread CTA runs out of registers)
+//   FRESCO_ATTN_POLY    0 (default) | 4 | 8: every n-th pair of exponentials by a polynomial on the FMA pipe
+//                       instead of MUFU.EX2
+//   FRESCO_ATTN_ROWSUM  64-key tiles only: row sums from the tensor core (one m64n8 wgmma of P against a tile of
+//                       ones per K step) instead of adds of the fp32 exponentials
+#include "common.cuh"
+#include "fresco_internal.h"
+
+namespace fresco {
+
+template <int D, int KN, int NWG, bool ROWSUM>
+struct AttnCfg {
+  static constexpr int TILE_M = 64 * NWG;             // query rows per CTA
+  static constexpr int THREADS = 128 * NWG + 32;
+  static constexpr int Q_ATOM = TILE_M * 128;         // [TILE_M rows x 64 fp16]
+  static constexpr int KV_ATOM = KN * 128;            // [KN rows x 64 fp16]
+  static constexpr int NATOM = (D + 63) / 64;
+  static constexpr int KSTEPS = (D + 15) / 16;
+  static constexpr int DPAD = KSTEPS * 16;
+  static constexpr int N0 = DPAD < 64 ? DPAD : 64;   // P V columns from atom 0
+  static constexpr int N1 = DPAD - N0;               // P V columns from atom 1
+  static constexpr int Q_BYTES = NATOM * Q_ATOM;
+  static constexpr int STAGE_BYTES = 2 * NATOM * KV_ATOM;
+  static constexpr int ONES_BYTES = ROWSUM ? 2048 : 0;  // [16 keys x 64] fp16 ones: B operand of the row-sum wgmma
+  static constexpr int FIXED = 1024 + Q_BYTES + ONES_BYTES + 256;
+  static constexpr int FIT = (227 * 1024 - FIXED) / STAGE_BYTES;
+  static constexpr int STAGES = FIT < 4 ? FIT : 4;
+  static constexpr int SMEM_BYTES = FIXED + STAGES * STAGE_BYTES;
+  static_assert(STAGES >= 2, "shared memory");
+};
+
+struct AttnParams {
+  __half* out;
+  int q_len, kv_len, heads, q_per_kv;
+  float scale_log2;        // softmax_scale * log2(e)
+  float diag_bias_log2;    // bias added where kv index == query index, * log2(e)
+};
+
+// exp2 on the FMA pipe (POLY variants): Cody-Waite split x = n + f, f in [-0.5, 0.5], degree-3 minimax polynomial for
+// 2^f (max relative error 7.5e-5, inside the fp16 rounding of P), exponent patched in with an integer add.
+__device__ __forceinline__ float exp2_poly(float t) {
+  t = fmaxf(t, -126.0f);
+  const float r = __fadd_rn(t, 12582912.0f);          // 1.5 * 2^23: the integer part lands in the low mantissa bits
+  const float f = __fsub_rn(t, __fsub_rn(r, 12582912.0f));
+  float q = fmaf(0.05517164617776871f, f, 0.2426111251115799f);
+  q = fmaf(q, f, 0.6932609677314758f);
+  q = fmaf(q, f, 0.9999280571937561f);
+  return __int_as_float(__float_as_int(q) + (__float_as_int(r) << 23));
+}
+
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+template <int D, int KN, int NWG, int POLY, bool ROWSUM>
+__global__ void __launch_bounds__(AttnCfg<D, KN, NWG, ROWSUM>::THREADS, 1)
+fresco_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
+                   const __grid_constant__ CUtensorMap tm_v, const AttnParams p) {
+  using Cfg = AttnCfg<D, KN, NWG, ROWSUM>;
+  constexpr int ST = Cfg::STAGES;
+  constexpr int kTileM = Cfg::TILE_M, kTileN = KN, kQAtomBytes = Cfg::Q_ATOM, kKVAtomBytes = Cfg::KV_ATOM;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* s_q = smem;
+  uint8_t* s_kv = smem + Cfg::Q_BYTES;
+  uint8_t* s_ones = s_kv + ST * Cfg::STAGE_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_ones + Cfg::ONES_BYTES);
+  uint64_t* bar_q = bars;
+  uint64_t* bar_full = bars + 1;               // [ST]
+  uint64_t* bar_empty = bars + 1 + ST;         // [ST] one arrival per consumer warp
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int q0 = blockIdx.x * kTileM;
+  const int head = blockIdx.y;
+  const int b = blockIdx.z;
+  const int b_kv = b / p.q_per_kv;
+  const int n_tiles = (p.kv_len + kTileN - 1) / kTileN;
+
+  if (threadIdx.x == 0) {
+    mbar_init(bar_q, 1);
+    for (int s = 0; s < ST; ++s) {
+      mbar_init(bar_full + s, 1);
+      mbar_init(bar_empty + s, 4 * NWG);
+    }
+    fence_barrier_init();
+  }
+  if (ROWSUM) {
+    for (int i = threadIdx.x; i < Cfg::ONES_BYTES / 4; i += Cfg::THREADS) reinterpret_cast<uint32_t*>(s_ones)[i] = 0x3C003C00u;
+    fence_proxy_async_smem();
+  }
+  __syncthreads();
+
+  if (warp == 4 * NWG) {
+    // ------------------------------------------------------------ TMA producer
+    if (FRESCO_ISSUER_THREAD(lane)) {
+      tma_prefetch_desc(&tm_q);
+      tma_prefetch_desc(&tm_k);
+      tma_prefetch_desc(&tm_v);
+      mbar_expect_tx(bar_q, Cfg::Q_BYTES);
+      for (int a = 0; a < Cfg::NATOM; ++a) tma_load_4d(s_q + a * kQAtomBytes, &tm_q, bar_q, a * 64, head, q0, b);
+      for (int t = 0; t < n_tiles; ++t) {
+        const int st = t % ST;
+        if (t >= ST) mbar_wait_mma_backoff(bar_empty + st, ((t / ST) - 1) & 1, 64);
+        uint8_t* sk = s_kv + st * Cfg::STAGE_BYTES;
+        uint8_t* sv = sk + Cfg::NATOM * kKVAtomBytes;
+        mbar_expect_tx(bar_full + st, Cfg::STAGE_BYTES);
+        for (int a = 0; a < Cfg::NATOM; ++a) {
+          tma_load_4d(sk + a * kKVAtomBytes, &tm_k, bar_full + st, a * 64, head, t * kTileN, b_kv);
+          tma_load_4d(sv + a * kKVAtomBytes, &tm_v, bar_full + st, a * 64, head, t * kTileN, b_kv);
+        }
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------- consumer warpgroups
+  const int wg = warp >> 2;
+  const int row0 = q0 + wg * 64 + acc_row(0);      // this thread's two query rows: row0, row0 + 8
+  const float scale_log2 = p.scale_log2, bias_log2 = p.diag_bias_log2;
+  const bool use_bias = bias_log2 != 0.f;
+  float o0[Cfg::N0 / 2], o1[Cfg::N1 > 0 ? Cfg::N1 / 2 : 1];
+#pragma unroll
+  for (int i = 0; i < Cfg::N0 / 2; ++i) o0[i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < (Cfg::N1 > 0 ? Cfg::N1 / 2 : 1); ++i) o1[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  float l_acc[4] = {0.f, 0.f, 0.f, 0.f};           // ROWSUM: every column of the m64n8 accumulator is the row sum
+  const uint32_t q_addr = smem_u32(s_q) + wg * 64 * 128;
+
+  mbar_wait_mma(bar_q, 0);
+  for (int t = 0; t < n_tiles; ++t) {
+    const int st = t % ST;
+    mbar_wait_mma(bar_full + st, (t / ST) & 1);
+    const uint32_t k_addr = smem_u32(s_kv + st * Cfg::STAGE_BYTES);
+    const uint32_t v_addr = k_addr + Cfg::NATOM * kKVAtomBytes;
+
+    // ---- S = Q K^T  (64 x 128 per warpgroup)
+    float s[kTileN / 2];
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < Cfg::KSTEPS; ++ks) {
+      const uint32_t qoff = (ks >> 2) * kQAtomBytes + (ks & 3) * 32;
+      const uint32_t koff = (ks >> 2) * kKVAtomBytes + (ks & 3) * 32;
+      wgmma_ss<kTileN>(s, make_smem_desc_sw128(q_addr + qoff, 16, 1024), make_smem_desc_sw128(k_addr + koff, 16, 1024),
+                       ks > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+
+    // ---- scale, mask the ragged tail, diagonal bias (all in the log2 domain)
+    const int col0 = t * kTileN;
+    const bool special = (col0 + kTileN > p.kv_len) || (use_bias && q0 < col0 + kTileN && q0 + kTileM > col0);
+#pragma unroll
+    for (int i = 0; i < kTileN / 2; ++i) s[i] *= scale_log2;
+    if (special) {
+#pragma unroll
+      for (int i = 0; i < kTileN / 2; ++i) {
+        const int col = col0 + acc_col(i);
+        const int row = row0 + 8 * ((i >> 1) & 1);
+        if (use_bias && col == row) s[i] += bias_log2;
+        if (col >= p.kv_len) s[i] = -INFINITY;
+      }
+    }
+    // ---- online softmax: row max over the quad, rescale O and l, p = exp2(s - m)
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < kTileN / 2; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
+    float alpha[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const float m_new = fmaxf(m_run[r], quad_max(mx[r]));
+      alpha[r] = fast_exp2(m_run[r] - m_new);
+      m_run[r] = m_new;
+      l_run[r] *= alpha[r];
+    }
+#pragma unroll
+    for (int i = 0; i < kTileN / 2; ++i) {
+      const float x = s[i] - m_run[(i >> 1) & 1];
+      s[i] = (POLY > 0 && ((i >> 1) % (POLY > 0 ? POLY : 1)) == POLY - 1) ? exp2_poly(x) : fast_exp2(x);
+      if (!ROWSUM) l_run[(i >> 1) & 1] += s[i];
+    }
+    if (ROWSUM) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) l_acc[i] *= alpha[(i >> 1) & 1];
+    }
+#pragma unroll
+    for (int i = 0; i < Cfg::N0 / 2; ++i) o0[i] *= alpha[(i >> 1) & 1];
+    if (Cfg::N1 > 0) {
+#pragma unroll
+      for (int i = 0; i < Cfg::N1 / 2; ++i) o1[i] *= alpha[(i >> 1) & 1];
+    }
+
+    // ---- O += P V: P (fp16) as register A fragments, 16 keys per step
+    uint32_t pa[kTileN / 16][4];
+#pragma unroll
+    for (int k2 = 0; k2 < kTileN / 16; ++k2)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) pa[k2][j] = pack_half2(s[8 * k2 + 2 * j], s[8 * k2 + 2 * j + 1]);
+    reg_fence(o0);
+    reg_fence(o1);
+    reg_fence(l_acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k2 = 0; k2 < kTileN / 16; ++k2) {
+      wgmma_rs<Cfg::N0>(o0, pa[k2], make_smem_desc_sw128(v_addr + k2 * 2048, kKVAtomBytes, 1024), 1u);
+      if constexpr (Cfg::N1 > 0)
+        wgmma_rs<Cfg::N1>(o1, pa[k2], make_smem_desc_sw128(v_addr + kKVAtomBytes + k2 * 2048, kKVAtomBytes, 1024), 1u);
+      if constexpr (ROWSUM)   // l += P_t * ones  (every element of the tile is 1.0, so its layout is moot)
+        wgmma_rs<8>(l_acc, pa[k2], make_smem_desc_sw128(smem_u32(s_ones), 2048, 1024), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o0);
+    reg_fence(o1);
+    reg_fence(l_acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar_empty + st);   // this warp's reads of K_t and V_t are complete
+  }
+
+  // ---- epilogue: O / l -> fp16 head slice of the two rows
+  float inv[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) inv[r] = 1.f / (ROWSUM ? l_acc[2 * r] : quad_sum(l_run[r]));
+  const size_t row_elems = static_cast<size_t>(p.heads) * D;
+  __half* dst = p.out + static_cast<size_t>(b) * p.q_len * row_elems + static_cast<size_t>(head) * D;
+#pragma unroll
+  for (int i = 0; i < Cfg::N0 / 2; i += 2) {
+    const int row = row0 + 8 * ((i >> 1) & 1), col = acc_col(i);
+    const float sc = inv[(i >> 1) & 1];
+    if (row < p.q_len && col < D)
+      *reinterpret_cast<uint32_t*>(dst + row * row_elems + col) = pack_half2(o0[i] * sc, o0[i + 1] * sc);
+  }
+  if constexpr (Cfg::N1 > 0) {
+#pragma unroll
+    for (int i = 0; i < Cfg::N1 / 2; i += 2) {
+      const int row = row0 + 8 * ((i >> 1) & 1), col = 64 + acc_col(i);
+      const float sc = inv[(i >> 1) & 1];
+      if (row < p.q_len && col < D)
+        *reinterpret_cast<uint32_t*>(dst + row * row_elems + col) = pack_half2(o1[i] * sc, o1[i + 1] * sc);
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// host side
+// ---------------------------------------------------------------------------------------------
+
+// {head_dim, heads, tokens, batch} view of a token-major [batch, tokens, heads*head_dim] fp16 tensor.
+// cuTensorMapEncodeTiled costs a few microseconds and the same (pointer, shape) comes back every denoise step (torch's
+// caching allocator), so encoded maps are kept in a small direct-mapped table.
+struct MapKey {
+  const void* base;
+  int head_dim, heads, tokens, batch, box_rows;
+  long long row_stride, batch_stride;
+  bool operator==(const MapKey& o) const {
+    return base == o.base && head_dim == o.head_dim && heads == o.heads && tokens == o.tokens && batch == o.batch &&
+           box_rows == o.box_rows && row_stride == o.row_stride && batch_stride == o.batch_stride;
+  }
+};
+// row_stride / batch_stride in elements (dense: heads*head_dim and tokens*heads*head_dim)
+static int make_head_tile_map(CUtensorMap* map, const void* base, int head_dim, int heads, int tokens, int batch,
+                              int box_rows, long long row_stride, long long batch_stride) {
+  constexpr int kSlots = 64;
+  static thread_local MapKey keys[kSlots];
+  static thread_local CUtensorMap maps[kSlots];
+  static thread_local bool valid[kSlots];
+  const MapKey key = {base, head_dim, heads, tokens, batch, box_rows, row_stride, batch_stride};
+  const size_t h = (reinterpret_cast<uintptr_t>(base) >> 9) * 0x9E3779B97F4A7C15ull + (size_t)tokens * 31 + box_rows;
+  const int slot = (int)((h >> 32) % kSlots);
+  if (valid[slot] && keys[slot] == key) {
+    *map = maps[slot];
+    return 0;
+  }
+  const cuuint64_t dims[4] = {(cuuint64_t)head_dim, (cuuint64_t)heads, (cuuint64_t)tokens, (cuuint64_t)batch};
+  const cuuint64_t strides[3] = {(cuuint64_t)head_dim * 2, (cuuint64_t)row_stride * 2, (cuuint64_t)batch_stride * 2};
+  const cuuint32_t box[4] = {64, 1, (cuuint32_t)box_rows, 1};
+  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  const int rc = encode_tiled_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box,
+                                  estr, CU_TENSOR_MAP_SWIZZLE_128B);
+  if (rc == 0) {
+    keys[slot] = key;
+    maps[slot] = *map;
+    valid[slot] = true;
+  }
+  return rc;
+}
+
+template <int D, int KN, int NWG, int POLY, bool ROWSUM>
+static int launch_variant(const void* q, const void* k, const void* v, void* out, int batch_q, int q_len, int kv_len,
+                          int heads, int q_per_kv, long long kv_row_stride, long long kv_batch_stride,
+                          const AttnParams& p, cudaStream_t stream) {
+  using Cfg = AttnCfg<D, KN, NWG, ROWSUM>;
+  CUtensorMap tq, tk, tv;
+  const int batch_kv = batch_q / q_per_kv;
+  const long long C = (long long)heads * D;
+  if (make_head_tile_map(&tq, q, D, heads, q_len, batch_q, Cfg::TILE_M, C, C * q_len)) return FRESCO_ERR_TENSORMAP;
+  if (make_head_tile_map(&tk, k, D, heads, kv_len, batch_kv, KN, kv_row_stride, kv_batch_stride)) return FRESCO_ERR_TENSORMAP;
+  if (make_head_tile_map(&tv, v, D, heads, kv_len, batch_kv, KN, kv_row_stride, kv_batch_stride)) return FRESCO_ERR_TENSORMAP;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(fresco_attn_kernel<D, KN, NWG, POLY, ROWSUM>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+    if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(attn)");
+    attr_set = true;
+  }
+  dim3 grid((q_len + Cfg::TILE_M - 1) / Cfg::TILE_M, heads, batch_q);
+  fresco_attn_kernel<D, KN, NWG, POLY, ROWSUM><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(tq, tk, tv, p);
+  return check_launch("fresco_attn_kernel");
+}
+
+// the variant the options select for a head dim (see the comment at the top of this file)
+struct AttnVariant {
+  int wide, poly, rowsum;
+};
+static AttnVariant attn_variant(int head_dim) {
+  AttnVariant a;
+  a.wide = option(OPT_ATTN_WIDE, 1);
+  a.wide = a.wide <= 0 ? 0 : (a.wide >= 2 && head_dim <= 64 ? 2 : 1);
+  a.poly = option(OPT_ATTN_POLY, 0);
+  a.poly = (a.poly == 4 || a.poly == 8) ? a.poly : 0;
+  a.rowsum = a.wide == 0 && option(OPT_ATTN_ROWSUM, 0) > 0;
+  return a;
+}
+
+template <int D, int KN, int NWG, bool ROWSUM>
+static int launch_poly(int poly, const void* q, const void* k, const void* v, void* out, int batch_q, int q_len,
+                       int kv_len, int heads, int q_per_kv, long long kv_row_stride, long long kv_batch_stride,
+                       const AttnParams& p, cudaStream_t s) {
+  if (poly == 4)
+    return launch_variant<D, KN, NWG, 4, ROWSUM>(q, k, v, out, batch_q, q_len, kv_len, heads, q_per_kv, kv_row_stride,
+                                                 kv_batch_stride, p, s);
+  if (poly == 8)
+    return launch_variant<D, KN, NWG, 8, ROWSUM>(q, k, v, out, batch_q, q_len, kv_len, heads, q_per_kv, kv_row_stride,
+                                                 kv_batch_stride, p, s);
+  return launch_variant<D, KN, NWG, 0, ROWSUM>(q, k, v, out, batch_q, q_len, kv_len, heads, q_per_kv, kv_row_stride,
+                                               kv_batch_stride, p, s);
+}
+
+template <int D>
+static int launch_attn(const void* q, const void* k, const void* v, void* out, int batch_q, int q_len, int kv_len,
+                       int heads, int q_per_kv, long long kv_row_stride, long long kv_batch_stride, float softmax_scale,
+                       float diag_bias, cudaStream_t stream) {
+  AttnParams p;
+  p.out = static_cast<__half*>(out);
+  p.q_len = q_len;
+  p.kv_len = kv_len;
+  p.heads = heads;
+  p.q_per_kv = q_per_kv;
+  p.scale_log2 = softmax_scale * 1.4426950408889634f;
+  p.diag_bias_log2 = diag_bias * 1.4426950408889634f;
+  const AttnVariant a = attn_variant(D);
+#define ATTN_ARGS q, k, v, out, batch_q, q_len, kv_len, heads, q_per_kv, kv_row_stride, kv_batch_stride, p, stream
+  if (a.wide == 0)
+    return a.rowsum ? launch_poly<D, 64, 2, true>(a.poly, ATTN_ARGS) : launch_poly<D, 64, 2, false>(a.poly, ATTN_ARGS);
+  if constexpr (D <= 64) {
+    if (a.wide == 2) return launch_poly<D, 128, 3, false>(a.poly, ATTN_ARGS);
+  }
+  return launch_poly<D, 128, 2, false>(a.poly, ATTN_ARGS);
+#undef ATTN_ARGS
+}
+
+}  // namespace fresco
+
+using namespace fresco;
+
+// which kernel fresco_attn_fwd launches for a head dim under the current options (bench.py names it in its JSON line)
+extern "C" const char* fresco_attn_variant(int head_dim) {
+  static thread_local char buf[96];
+  const AttnVariant a = attn_variant(head_dim);
+  snprintf(buf, sizeof(buf), "fresco_attn_kernel<%d,keys%d,wg%d,poly%d%s> (wgmma)", head_dim, a.wide == 0 ? 64 : 128,
+           a.wide == 2 ? 3 : 2, a.poly, a.rowsum ? ",rowsum" : "");
+  return buf;
+}
+
+extern "C" int fresco_attn_fwd(const void* q, const void* k, const void* v, void* out, int batch_q, int q_len,
+                               int kv_len, int heads, int head_dim, int q_per_kv, float softmax_scale,
+                               float diag_bias, void* stream) {
+  return fresco_attn_fwd_kv_strided(q, k, v, out, batch_q, q_len, kv_len, heads, head_dim, q_per_kv,
+                                    (long long)heads * head_dim, (long long)kv_len * heads * head_dim, softmax_scale,
+                                    diag_bias, stream);
+}
+
+extern "C" int fresco_attn_fwd_kv_strided(const void* q, const void* k, const void* v, void* out, int batch_q, int q_len,
+                                          int kv_len, int heads, int head_dim, int q_per_kv, long long kv_row_stride,
+                                          long long kv_batch_stride, float softmax_scale, float diag_bias, void* stream) {
+  if (!q || !k || !v || !out) return set_error(FRESCO_ERR_ARG, "fresco_attn_fwd: null pointer");
+  if (batch_q <= 0 || q_len <= 0 || kv_len <= 0 || heads <= 0 || q_per_kv <= 0 || batch_q % q_per_kv != 0)
+    return set_error(FRESCO_ERR_ARG, "fresco_attn_fwd: bad shape");
+  if (kv_row_stride < (long long)heads * head_dim || kv_row_stride % 8 != 0 || kv_batch_stride % 8 != 0 ||
+      kv_batch_stride < kv_row_stride)
+    return set_error(FRESCO_ERR_ARG, "fresco_attn_fwd: K/V strides must be multiples of 8 elements and cover a row");
+  if (softmax_scale <= 0.f) return set_error(FRESCO_ERR_ARG, "fresco_attn_fwd: softmax_scale must be > 0");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+#define ATTN_CASE(DD)                                                                                                 \
+  case DD:                                                                                                             \
+    return launch_attn<DD>(q, k, v, out, batch_q, q_len, kv_len, heads, q_per_kv, kv_row_stride, kv_batch_stride,      \
+                           softmax_scale, diag_bias, s)
+  switch (head_dim) {
+    ATTN_CASE(40);
+    ATTN_CASE(64);
+    ATTN_CASE(80);
+    ATTN_CASE(128);
+    default: return set_error(FRESCO_ERR_UNSUPPORTED, "fresco_attn_fwd: head_dim must be one of 40, 64, 80, 128");
+  }
+#undef ATTN_CASE
+}

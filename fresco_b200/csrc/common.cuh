@@ -1,13 +1,14 @@
-// Thin inline-PTX wrappers for the sm_100a features the kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / st).
-// Bit layouts of the UMMA descriptors follow the PTX ISA "tcgen05 matrix
-// descriptor" / "instruction descriptor" tables.
+// Thin inline-PTX wrappers for the sm_90a features the kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / commit / wait; the MMAs themselves are in wgmma.cuh).
+// The bit layout of the matrix descriptor follows the PTX ISA "wgmma matrix descriptor" table.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+
+#include "wgmma.cuh"
 
 namespace fresco {
 
@@ -25,16 +26,9 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
-// The single thread of a warp that issues TMA / tcgen05.mma / tcgen05.commit.  Selecting it with elect.sync (and not
-// with `lane == 0`) matters: the compiler then knows that exactly one thread runs the branch and keeps descriptors and
-// TMEM addresses in uniform registers; behind `lane == 0` every UTCHMMA / UTMALDG is wrapped in a
-// vote-and-broadcast loop (ELECT / R2UR.BROADCAST / BRA.U.ANY), which cost the issuing thread 60-70 clocks per
-// instruction in round 1's traces.  -DFRESCO_ISSUER_LANE0 restores the old form for A/B measurements.
-#ifdef FRESCO_ISSUER_LANE0
-#define FRESCO_ISSUER_THREAD(lane) ((lane) == 0)
-#else
+// The single thread of a warp that issues TMA.  Selecting it with elect.sync (and not with `lane == 0`) lets the
+// compiler keep the tensor-map and barrier addresses in uniform registers.
 #define FRESCO_ISSUER_THREAD(lane) (::fresco::elect_one())
-#endif
 
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -53,9 +47,8 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// try_wait suspends the thread until the phase completes or a time limit passes.  The default limit is short: round-2
-// profiles show softmax warps going round the poll loop 2-5 times per tile (9 instructions each, in competition with
-// the warps that do have work for the same issue slots).  The hint asks for up to FRESCO_TRYWAIT_NS before giving up;
+// try_wait suspends the thread until the phase completes or a time limit passes.  The hint asks for up to
+// FRESCO_TRYWAIT_NS before giving up, so a waiting warp does not take issue slots from the warps that have work;
 // completion still wakes the thread at once.
 #ifndef FRESCO_TRYWAIT_NS
 #define FRESCO_TRYWAIT_NS 2000
@@ -108,6 +101,21 @@ __device__ __forceinline__ void mbar_wait_backoff(uint64_t* bar, uint32_t parity
     if (++polls > FRESCO_WATCHDOG_POLLS) mbar_timeout(bar, parity, tag);
   }
 }
+// Kernels that issue wgmma use these instead: ptxas serialises every wgmma of a kernel that contains a call to a function
+// that is not inlined (mbar_timeout and its printf), so their watchdog traps without a report.
+__device__ __forceinline__ void mbar_wait_mma(uint64_t* bar, uint32_t parity) {
+  uint32_t polls = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++polls > FRESCO_WATCHDOG_POLLS) __trap();
+  }
+}
+__device__ __forceinline__ void mbar_wait_mma_backoff(uint64_t* bar, uint32_t parity, uint32_t ns) {
+  uint32_t polls = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    __nanosleep(ns);
+    if (++polls > FRESCO_WATCHDOG_POLLS) __trap();
+  }
+}
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
@@ -131,102 +139,37 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot_in_smem) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)),
-               "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---------------------------------------------------------------- wgmma
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving reads or writes of accumulator registers across an asynchronous wgmma
+template <int N>
+__device__ __forceinline__ void reg_fence(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once every previously issued tcgen05.mma has completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// 32 lanes x 32 consecutive 32-bit columns -> 32 registers per thread
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ---------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor (64 bit):
+// wgmma shared-memory matrix descriptor (64 bit):
 //   [0,14) start address >> 4   [16,30) leading byte offset >> 4   [32,46) stride byte offset >> 4
-//   [46,48) version = 1 (sm_100)  [49,52) base offset  [61,64) swizzle (2 = 128B)
+//   [49,52) base offset  [62,64) layout (1 = 128B swizzle)
+// K-major operands: SBO = 1024 (eight 128-byte rows), LBO unused.  MN-major operands: LBO = distance between 64-element
+// column blocks, SBO = 1024.  A K step of 16 inside a K-major 128B-swizzled atom adds 32 bytes to the start address.
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
                                                          uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// Instruction descriptor (32 bit) for kind::f16, fp16 A/B, fp32 accumulate:
-//   [4,6) D format (1 = f32)  [7,10) A format (0 = f16)  [10,13) B format
-//   [15] A major (0 = K)  [16] B major (0 = K, 1 = MN)  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, int b_mn_major) {
-  return (1u << 4) | (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
-}
+
+// (row, column) inside a warpgroup's 64 x N wgmma accumulator of accumulator register i (see wgmma.cuh)
+__device__ __forceinline__ int acc_row(int i) { return 16 * ((threadIdx.x >> 5) & 3) + ((threadIdx.x & 31) >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int acc_col(int i) { return 8 * (i >> 2) + 2 * (threadIdx.x & 3) + (i & 1); }
 
 __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   __half2 h = __floats2half2_rn(lo, hi);

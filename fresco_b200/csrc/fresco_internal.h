@@ -22,7 +22,7 @@ int sm_count();
 
 // Tuning options: each has the name of an environment variable, which is read ONCE (first use); fresco_set_option()
 // overrides it afterwards (tests, tools).  Nothing on a launch path calls getenv.
-enum Option { OPT_ATTN_WIDE = 0, OPT_ATTN_POLY, OPT_ATTN_ROWSUM, OPT_ATTN_ABLATE, OPT_TEMPORAL_V, OPT_GRAM_V, OPT_COUNT };
+enum Option { OPT_ATTN_WIDE = 0, OPT_ATTN_POLY, OPT_ATTN_ROWSUM, OPT_TEMPORAL_V, OPT_GRAM_V, OPT_COUNT };
 int option(Option which, int dflt);
 
 }  // namespace fresco

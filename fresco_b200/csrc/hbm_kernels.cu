@@ -1632,7 +1632,7 @@ static bool quad_config(int hw, int channels, int planes, int bytes_per_px, int&
   for (NQ = 4; NQ >= 1; NQ >>= 1) {
     if (channels % (4 * NQ) != 0) continue;
     if ((size_t)NQ * hw * bytes_per_px > 200 * 1024) continue;
-    if (NQ > 1 && planes / (4 * NQ) < 148) continue;                 // keep every SM busy
+    if (NQ > 1 && planes / (4 * NQ) < sm_count()) continue;           // keep every SM busy
     P = 4 / NQ;                                                       // P * NQ == 4 carried float4 per thread
     T = ((hw + P - 1) / P + 31) / 32 * 32;
     while (T > 1024 && P * NQ < 4 * 4) {                              // large planes: more pixels per thread

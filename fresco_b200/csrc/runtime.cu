@@ -66,7 +66,7 @@ int encode_tiled_map(CUtensorMap* map, CUtensorMapDataType dtype, int rank, void
 }
 
 static const char* const kOptionNames[OPT_COUNT] = {"FRESCO_ATTN_WIDE", "FRESCO_ATTN_POLY", "FRESCO_ATTN_ROWSUM",
-                                                    "FRESCO_ATTN_ABLATE", "FRESCO_TEMPORAL_V", "FRESCO_GRAM_V"};
+                                                    "FRESCO_TEMPORAL_V", "FRESCO_GRAM_V"};
 static std::atomic<int> g_opt_state[OPT_COUNT];      // 0 = not looked at, 1 = unset (use the default), 2 = set
 static std::atomic<int> g_opt_value[OPT_COUNT];
 

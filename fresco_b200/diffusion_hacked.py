@@ -8,7 +8,7 @@ Same public names, arguments and error behaviour as the reference (SURVEY 8b):
 * ``optimize_feature``          (:416-488)
 * ``my_forward`` / ``apply_FRESCO_opt`` / ``disable_FRESCO_opt``   (:491-831)
 
-The arithmetic of the hot path runs in libfresco_b200.so (hand-written sm_100a
+The arithmetic of the hot path runs in libfresco_b200.so (hand-written sm_90a
 kernels bound through ctypes); there is no PyTorch fallback for it.  What stays
 in torch is what the scope table leaves there: the Linear projections
 (to_q/k/v/out, cuBLAS) and small per-call tensor preparation.

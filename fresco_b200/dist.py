@@ -1,6 +1,6 @@
 """Frame-sharded FRESCO attention for one multi-GPU box (NCCL over NVLink / NVSwitch).
 
-The reference has no collective on this path (SURVEY 2.1); this module is the B200 design for BASELINE config 4: the
+The reference has no collective on this path (SURVEY 2.1); this module is the multi-GPU design for BASELINE config 4: the
 N keyframes of ONE batch are split contiguously over G ranks (rank r owns frames [r*N/G, (r+1)*N/G) of both CFG
 chunks) and the UNet body runs as plain replicas.  Only FRESCO attention couples frames:
 
@@ -61,7 +61,7 @@ class RingComm:
 
 
 class _OpsBackend:
-    """the product path: hand-written sm_100a kernels"""
+    """the product path: hand-written sm_90a kernels"""
 
     def kv_compact_packed(self, k, v, idx, kv_out, chunks):
         from . import ops

@@ -1,5 +1,5 @@
 """Drop-in for the reference's ``src/flow_utils.py`` + the geometry helpers it
-uses, backed by the sm_100a kernels (no PyTorch fallback for the hot ops).
+uses, backed by the sm_90a kernels (no PyTorch fallback for the hot ops).
 
 Public names and argument meaning follow the reference:
 ``warp_tensor`` (src/flow_utils.py:18-53), ``get_single_mapping_ind`` (:56-102),

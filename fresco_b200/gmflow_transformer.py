@@ -5,7 +5,7 @@
   attentions of the feature transformer (6 blocks x self / cross; 2 x 2 windows of 32 x 32 tokens at 512 x 512, C = 128)
 * ``feature_flow_attention(module, feature0, flow)``            (:353-374) -- flow propagation, V = the 2-channel flow
 
-All three run on the tcgen05 attention kernels of libfresco_b200.so (head_dim = C, one head, fp16 operands / fp32
+All three run on the wgmma attention kernel of libfresco_b200.so (head_dim = C, one head, fp16 operands / fp32
 softmax; SURVEY 9 measured fp16 operands adequate for GMFlow's LayerNorm-scale features).  The shifted-window variant
 does not add the reference's -100 mask to a dense score matrix: a masked pair contributes exp(-100) ~ 4e-44 of its row,
 i.e. nothing in fp32, so each window is split into the (up to four) regions inside which tokens may attend each other,

@@ -1,4 +1,4 @@
-/* fresco_b200 -- C ABI of the B200-native FRESCO hot path (libfresco_b200.so).
+/* fresco_b200 -- C ABI of the H100-native (sm_90a) FRESCO hot path (libfresco_b200.so).
  *
  * The reference (williamyang1991/FRESCO) has no FFI on this path: its boundary is a Python
  * monkey-patch surface over diffusers (SURVEY.md 8b).  The host side of this repo
@@ -36,7 +36,7 @@ const char* fresco_last_error(void);
 /* number of kernels launched by this library in this process (for bench.py's gpu_launches) */
 long long fresco_launch_count(void);
 /* tuning option by the name of its environment variable (FRESCO_ATTN_WIDE, FRESCO_ATTN_POLY, FRESCO_ATTN_ROWSUM,
- * FRESCO_ATTN_ABLATE, FRESCO_TEMPORAL_V, FRESCO_GRAM_V); the environment is read once, this overrides it;
+ * FRESCO_TEMPORAL_V, FRESCO_GRAM_V); the environment is read once, this overrides it;
  * value < 0 restores the built-in default. */
 int fresco_set_option(const char* name, int value);
 /* name of the kernel fresco_attn_fwd launches for a head dim under the current options (thread-local string) */
@@ -60,7 +60,7 @@ int fresco_rows_gather(const void* src, const int32_t* idx, void* dst, long long
                        int dst_stride_bytes, int dst_offset_bytes, void* stream);
 int fresco_rows_scatter(const void* src, const int32_t* idx, void* dst, long long n_rows, int row_bytes, void* stream);
 
-/* ---- A3 / A4: dense attention forward (tcgen05 + TMEM + TMA) -------------------------------
+/* ---- A3 / A4: dense attention forward (wgmma + TMA) ---------------------------------------
  * replaces F.scaled_dot_product_attention at src/diffusion_hacked.py:281-285 (spatial-guided:
  * q = to_q(ref), k = to_k(ref), v = current query, softmax_scale = 0.2/sqrt(d), diag_bias =
  * intraattn_bias) and :303-305 (cross-frame: shared compacted K/V, q_per_kv = frames).
@@ -142,10 +142,10 @@ int fresco_warp_loss_fwd_bwd_halo(const float* cs, const float* fwd_flow, const 
  * replaces src/diffusion_hacked.py:469-476 and its backward.
  * step 1  fresco_gram_normalize: cs float [batch, channels, tokens] -> xhat half [batch, tokens, channels]
  *         (row-normalised, token-major) and norms float [batch, tokens].
- * step 2  fresco_gram_sign (tcgen05): G = xhat xhat^T per batch; T = sign(G - A) + sign(G - A^T)
+ * step 2  fresco_gram_sign (wgmma): G = xhat xhat^T per batch; T = sign(G - A) + sign(G - A^T)
  *         written as half [batch, tokens, tokens]; loss += weight/(batch*tokens^2) * sum|G - A|.
  *         target float [batch, tokens, tokens] is the reference's correlation_matrix entry.
- * step 3  fresco_gram_grad (tcgen05): ghat = T xhat * weight/(batch*tokens^2), projected through the
+ * step 3  fresco_gram_grad (wgmma): ghat = T xhat * weight/(batch*tokens^2), projected through the
  *         normalisation Jacobian and added to grad float [batch, channels, tokens].             */
 int fresco_gram_normalize(const float* cs, void* xhat, float* norms, int batch, int channels, int tokens,
                           void* stream);

@@ -1,7 +1,7 @@
 """TEST / BENCH INFRASTRUCTURE ONLY -- the reference's math in PyTorch eager ON THE GPU.
 
 bench.py's ``gpu_eager_baseline`` leg: what the reference itself executes on a CUDA device (SURVEY 8d: "time the
-reference on the same B200 in PyTorch eager -- that, not the CPU number, is the >= 10x bar"), restated with the same
+reference on the same GPU in PyTorch eager -- that, not the CPU number, is the >= 10x bar"), restated with the same
 torch calls the reference makes (F.scaled_dot_product_attention, boolean-mask indexing + repeat, torch.gather,
 F.grid_sample, fp32 bmm, autograd + torch.optim.Adam), fp16 activations for attention as shipped
 (run_fresco.py:75-76), fp32 inside optimize_feature (diffusion_hacked.py:430).  Never imported by the product path.

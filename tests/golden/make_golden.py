@@ -1,14 +1,14 @@
-"""Generate golden vectors by running the REAL reference (/root/reference) on CPU.
+"""Generate golden vectors by running the REAL reference (williamyang1991/FRESCO) on CPU.
 
-Run in the build container only (the reference is not present on the GPU box):
-
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py [--set b] --reference /path/to/FRESCO
 
 The reference imports two diffusers names and matplotlib at module top
 (src/diffusion_hacked.py:7-8, src/utils.py:5); neither is used on the path we
 exercise, so they are stubbed in ``sys.modules``.  Outputs: small ``.npz``
 fixtures next to this script, consumed by tests/test_oracle_golden.py (oracle
-vs reference) and by the ``-m gpu`` parity tests.
+vs reference) and by the ``-m gpu`` parity tests.  A fixture whose compressed size
+would pass 1 MB is stored in parts (``name.npz``, ``name.1.npz``, ...) that the
+``golden`` fixture of tests/conftest.py merges again.
 """
 import os
 import sys
@@ -19,7 +19,32 @@ import torch
 import torch.nn.functional as F
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = "/root/reference"
+REF = sys.argv[sys.argv.index("--reference") + 1] if "--reference" in sys.argv else None
+PART_BYTES = 960 * 1024
+
+
+def save_npz(name, **arrays):
+    """savez_compressed into HERE/name.npz, split by array into parts below PART_BYTES each."""
+    import io
+    import zipfile
+    for old in os.listdir(HERE):
+        if old.startswith(name + ".") and old.endswith(".npz"):
+            os.remove(os.path.join(HERE, old))
+    sizes = {}
+    for k, v in arrays.items():
+        buf = io.BytesIO()
+        np.savez_compressed(buf, **{k: v})
+        sizes[k] = zipfile.ZipFile(buf).infolist()[0].compress_size + 256
+    parts, cur, used = [], {}, 0
+    for k, v in arrays.items():
+        if cur and used + sizes[k] > PART_BYTES:
+            parts.append(cur)
+            cur, used = {}, 0
+        cur[k] = v
+        used += sizes[k]
+    parts.append(cur)
+    for i, part in enumerate(parts):
+        np.savez_compressed(os.path.join(HERE, name + (".npz" if i == 0 else ".%d.npz" % i)), **part)
 
 
 def import_reference():
@@ -154,7 +179,7 @@ def scenario_b(dh, fu, geometry, matching, ut):
     finally:
         torch.optim.Adam.step = orig_step
     res.update(opt_sample=sample.numpy(), opt_target=target.numpy())
-    np.savez_compressed(os.path.join(HERE, "set_b.npz"), **res)
+    save_npz("set_b", **res)
     print("golden fixture set B written to", HERE)
 
 
@@ -170,8 +195,7 @@ def main():
     fwd, bwd = smooth_flows(N, H, W, 1, 3.0)
     fo, bo = geometry.forward_backward_consistency_check(fwd, bwd)
     feat = torch.randn(N, 5, H, W)
-    np.savez_compressed(os.path.join(HERE, "geometry.npz"),
-                        fwd=fwd.numpy(), bwd=bwd.numpy(), fwd_occ=fo.numpy(), bwd_occ=bo.numpy(),
+    save_npz("geometry", fwd=fwd.numpy(), bwd=bwd.numpy(), fwd_occ=fo.numpy(), bwd_occ=bo.numpy(),
                         feat=feat.numpy(), warped=geometry.flow_warp(feat, bwd).numpy())
 
     # ---------------- mapping (integer path) ----------------
@@ -186,7 +210,7 @@ def main():
         out.update({f"{tag}_bwd_flows": b_.numpy(), f"{tag}_bwd_occs": bo_.numpy(), f"{tag}_imgs": im_.numpy(),
                     f"{tag}_scale": np.float32(sc), f"{tag}_fwd_map": fm.numpy(), f"{tag}_bwd_map": bm.numpy(),
                     f"{tag}_mask": im.numpy(), f"{tag}_single_map": mp.numpy(), f"{tag}_single_unl": unl.numpy()})
-    np.savez_compressed(os.path.join(HERE, "mapping.npz"), **out)
+    save_npz("mapping", **out)
 
     # ---------------- attention, all 8 flag combinations ----------------
     C, heads, chunks = 80, 2, 2
@@ -224,14 +248,13 @@ def main():
     proc = dh.FRESCOAttnProcessor2_0(chunks, ctrl)
     ctrl.enable_cfattn([attn_mask[1]])
     res["out_cf_nomask"] = proc(attn, x.clone()).numpy()
-    np.savez_compressed(os.path.join(HERE, "attention.npz"), **res)
+    save_npz("attention", **res)
 
     # ---------------- warp_tensor ----------------
     sal = torch.rand(N, 1, 32, 32)
     s_feat = torch.randn(2 * N, 6, 8, 8)
     s_img = torch.randn(N, 3, H, W)
-    np.savez_compressed(
-        os.path.join(HERE, "warp_tensor.npz"), fwd=fwd.numpy(), bwd=bwd.numpy(), fwd_occ=fo.numpy(),
+    save_npz("warp_tensor", fwd=fwd.numpy(), bwd=bwd.numpy(), fwd_occ=fo.numpy(),
         bwd_occ=bocc.numpy(), saliency=sal.numpy(), sample_feat=s_feat.numpy(), sample_img=s_img.numpy(),
         out_feat=fu.warp_tensor(s_feat.clone(), [fwd, bwd], [fo, bocc], sal, 2).numpy(),
         out_img=fu.warp_tensor(s_img.clone(), [fwd, bwd], [fo, bocc], sal, 1).numpy())
@@ -268,14 +291,14 @@ def main():
     torch.optim.Adam.step = orig_step
     opt["adain_out"] = ut.adaptive_instance_normalization(other, sample).numpy()
     opt["adain_content"] = other.numpy()
-    np.savez_compressed(os.path.join(HERE, "optimize.npz"), **opt)
+    save_npz("optimize", **opt)
 
     # ---------------- GMFlow global correlation ----------------
     f0 = torch.randn(2, 16, 6, 8)
     f1 = torch.roll(f0, shifts=(1, -2), dims=(2, 3)) * 3 + 0.3 * torch.randn(2, 16, 6, 8)
     flow_b, prob_b = matching.global_correlation_softmax(f0, f1, pred_bidir_flow=True)
     flow_u, _ = matching.global_correlation_softmax(f0, f1, pred_bidir_flow=False)
-    np.savez_compressed(os.path.join(HERE, "gmflow_corr.npz"), f0=f0.numpy(), f1=f1.numpy(),
+    save_npz("gmflow_corr", f0=f0.numpy(), f1=f1.numpy(),
                         flow_bidir=flow_b.numpy(), flow_uni=flow_u.numpy(), prob_bidir=prob_b.numpy())
     scenario_gmflow_attention()
     scenario_ddpm_step()
@@ -316,7 +339,7 @@ def scenario_ddpm_step():
     m = (torch.rand(3, 1, 40, 56, generator=g) > 0.9).float()
     res.update(dil_in=m.numpy(), dil5=ut.Dilate(kernel_size=5, device="cpu")(m).numpy(),
                dil13=ut.Dilate(kernel_size=13, device="cpu")(m).numpy())
-    np.savez_compressed(os.path.join(HERE, "ddpm_step.npz"), **res)
+    save_npz("ddpm_step", **res)
 
 
 def scenario_gmflow_attention():
@@ -345,7 +368,7 @@ def scenario_gmflow_attention():
         res.update(ffa_f0=f0.half().numpy(), ffa_flow=flow.numpy(), ffa_out=ffa(f0, flow).numpy(),
                    ffa_wq=ffa.q_proj.weight.numpy(), ffa_bq=ffa.q_proj.bias.numpy(), ffa_wk=ffa.k_proj.weight.numpy(),
                    ffa_bk=ffa.k_proj.bias.numpy())
-    np.savez_compressed(os.path.join(HERE, "gmflow_attn.npz"), **res)
+    save_npz("gmflow_attn", **res)
 
 
 if __name__ == "__main__":

@@ -2,16 +2,15 @@
 the host-side mirror of the reference's hook surface behaves like the reference, and the
 product path refuses to run without CUDA (no silent fallback)."""
 import ctypes
+import json
 import os
 import re
 import sys
-import types
 
 import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
 
 
 @pytest.fixture(scope="module")
@@ -44,27 +43,28 @@ def test_argument_errors_do_not_touch_the_gpu(built_lib):
 
 
 def test_default_attention_kernel_per_head_dim(built_lib):
-    """Host-side kernel selection through the C ABI (no launch): the measured-best kernel per head_dim is the default,
-    the options select the other parity-tested variants, negative values restore the defaults, unknown names fail."""
+    """Host-side kernel selection through the C ABI (no launch): the default variant per head_dim, the options select
+    the other parity-tested variants, negative values restore the defaults, unknown names fail."""
     l = built_lib.lib()
-    names = ("FRESCO_ATTN_WIDE", "FRESCO_ATTN_POLY")
+    names = ("FRESCO_ATTN_WIDE", "FRESCO_ATTN_POLY", "FRESCO_ATTN_ROWSUM")
     for n in names:
         assert l.fresco_set_option(n.encode(), -1) == 0
     v = lambda d: l.fresco_attn_variant(d).decode()
-    assert v(40) == "fresco_attn_twin_kernel<40,poly8,2>"          # two threads per row at the dominant FRESCO shape
-    assert v(80) == "fresco_attn_twin_kernel<80,poly4,1>"
-    assert v(64).startswith("fresco_attn_kernel<64,poly0>") and v(128).startswith("fresco_attn_kernel<128,poly0>")
+    for d in (40, 64, 80, 128):
+        assert v(d) == "fresco_attn_kernel<%d,keys128,wg2,poly0> (wgmma)" % d
     try:
-        assert l.fresco_set_option(b"FRESCO_ATTN_WIDE", 1) == 0 and l.fresco_set_option(b"FRESCO_ATTN_POLY", 0) == 0
-        assert v(40) == "fresco_attn_twin_kernel<40,poly0,1>" and v(64) == "fresco_attn_twin_kernel<64,poly0,1>"
-        assert v(128).startswith("fresco_attn_kernel<128")          # the twin kernel stops at head_dim 80
-        assert l.fresco_set_option(b"FRESCO_ATTN_WIDE", 0) == 0
-        assert v(40).startswith("fresco_attn_kernel<40,poly0>")
+        assert l.fresco_set_option(b"FRESCO_ATTN_WIDE", 2) == 0 and l.fresco_set_option(b"FRESCO_ATTN_POLY", 8) == 0
+        assert v(40) == "fresco_attn_kernel<40,keys128,wg3,poly8> (wgmma)"
+        assert v(80) == "fresco_attn_kernel<80,keys128,wg2,poly8> (wgmma)"      # three warpgroups stop at head_dim 64
+        assert l.fresco_set_option(b"FRESCO_ATTN_ROWSUM", 1) == 0
+        assert v(64) == "fresco_attn_kernel<64,keys128,wg3,poly8> (wgmma)"      # row sums: 64-key tiles only
+        assert l.fresco_set_option(b"FRESCO_ATTN_WIDE", 0) == 0 and l.fresco_set_option(b"FRESCO_ATTN_POLY", 4) == 0
+        assert v(128) == "fresco_attn_kernel<128,keys64,wg2,poly4,rowsum> (wgmma)"
         assert l.fresco_set_option(b"FRESCO_NO_SUCH_OPTION", 1) == -1
     finally:
         for n in names:
             l.fresco_set_option(n.encode(), -1)
-    assert v(40) == "fresco_attn_twin_kernel<40,poly8,2>"
+    assert v(40) == "fresco_attn_kernel<40,keys128,wg2,poly0> (wgmma)"
 
 
 def test_no_cpu_fallback(built_lib):
@@ -87,35 +87,16 @@ def test_product_never_imports_oracle():
                 assert "import oracle" not in src and "from oracle" not in src, os.path.join(dp, f)
 
 
-def _import_reference():
-    for name, attrs in (("diffusers", {}), ("diffusers.models", {}),
-                        ("diffusers.models.unet_2d_condition", {"UNet2DConditionOutput": object}),
-                        ("diffusers.models.attention_processor", {"AttnProcessor2_0": object}),
-                        ("matplotlib", {}), ("matplotlib.pyplot", {})):
-        if name not in sys.modules:
-            m = types.ModuleType(name)
-            for k, v in attrs.items():
-                setattr(m, k, v)
-            sys.modules[name] = m
-    cwd = os.getcwd()
-    os.chdir(REF)
-    sys.path.insert(0, REF)
-    try:
-        import src.diffusion_hacked as dh
-    finally:
-        os.chdir(cwd)
-    return dh
-
-
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not present")
 def test_attention_control_state_machine_matches_reference():
-    """drive the reference's AttentionControl and ours through the same call sequence"""
-    ref_dh = _import_reference()
+    """drive our AttentionControl through the call sequence recorded from the reference's AttentionControl
+    (tests/golden/attention_control.json: the state after every call, what each __call__ returned, the constants)"""
     from fresco_b200 import diffusion_hacked as my_dh
-    a, b = ref_dh.AttentionControl(), my_dh.AttentionControl()
+    with open(os.path.join(ROOT, "tests", "golden", "attention_control.json")) as f:
+        rec = json.load(f)
+    b = my_dh.AttentionControl()
 
     def snap(c):
-        return (c.store, c.index, c.use_intraattn, c.use_interattn, c.use_cfattn, len(c.stored_attn["decoder_attn"]))
+        return [c.store, c.index, c.use_intraattn, c.use_interattn, c.use_cfattn, len(c.stored_attn["decoder_attn"])]
 
     t = [torch.full((1,), float(i)) for i in range(6)]
     seq = [("enable_controller", ()), ("enable_store", ()), ("call", (t[0],)), ("call", (t[1],)), ("call", (t[2],)),
@@ -124,16 +105,16 @@ def test_attention_control_state_machine_matches_reference():
            ("enable_interattn", ({"fwd_mappings": [1]},)), ("disable_interattn", ()), ("enable_interattn", ()),
            ("disable_controller", ()), ("enable_controller", ()), ("clear_store", ()), ("enable_intraattn", ()),
            ("call", (t[3],))]
-    for name, args in seq:
+    assert [n for n, _ in seq] == [s["op"] for s in rec["steps"]]
+    for (name, args), want in zip(seq, rec["steps"]):
         if name == "call":
-            ra, rb = a(*args), b(*args)
-            assert (ra is None and rb is None) or torch.equal(ra, rb)
+            rb = b(*args)
+            assert (rb is None and want["returned"] is None) or rb.tolist() == want["returned"]
         else:
-            getattr(a, name)(*args)
             getattr(b, name)(*args)
-        assert snap(a) == snap(b), (name, snap(a), snap(b))
-    for attr in ("intraattn_bias", "intraattn_scale_factor", "interattn_scale_factor"):
-        assert getattr(a, attr) == getattr(b, attr)
+        assert snap(b) == want["state"], (name, snap(b), want["state"])
+    for attr, value in rec["attrs"].items():
+        assert getattr(b, attr) == value
 
 
 def test_hook_surface_on_harness_unet():

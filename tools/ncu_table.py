@@ -1,6 +1,6 @@
 """Compact per-launch table from an `ncu --set full` report (run where ncu is installed; no GPU needed):
 
-    python tools/ncu_table.py gpurun_out/r02_kernels.ncu-rep > profiles/r02_kernels_ncu.txt
+    python tools/ncu_table.py report.ncu-rep > kernels_ncu.txt
 
 One row per profiled launch: duration, DRAM bytes read + written (the `traffic` of the roofline object), DRAM / tensor /
 MUFU (XU) pipe utilisation, issue-slot utilisation, achieved occupancy, registers, dynamic shared memory, grid / block.
