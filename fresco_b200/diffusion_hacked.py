@@ -589,47 +589,68 @@ def gram_targets(features: Sequence[torch.Tensor], dense: bool = False):
 
 
 @torch.no_grad()
-def get_intraframe_paras(pipe, imgs, frescoProc, prompt_embeds, do_classifier_free_guidance=True, seed=0):
+def get_intraframe_paras(pipe, imgs, frescoProc, prompt_embeds, do_classifier_free_guidance=True, seed=0, shard=None):
     """Parameters for spatial-guided attention / optimisation (src/diffusion_hacked.py:843-901): one UNet pass
     on the noised input frames with the controller in store mode (fills
     ``frescoProc.controller.stored_attn['decoder_attn']``), then the normalised-Gram targets of the four
-    decoder features."""
+    decoder features.
+
+    ``shard=(world, rank[, group])`` (not in the reference): ``imgs`` / ``prompt_embeds`` hold ALL N frames; the
+    initial noise is drawn for all of them from the seeded generator and this rank's frames [rank*N/G, (rank+1)*N/G)
+    are sliced, encoded and run through the store pass.  The controller then holds this rank's reference inputs and
+    the targets cover this rank's frames (both CFG chunks): what the sharded processor and
+    ``optimize_feature(shard=...)`` take.  The pass is per frame, so no collective is issued."""
+    from .dist import chunk_frames, shard_frames
     scheduler = pipe.scheduler
     timestep = scheduler.timesteps[-1]
     device = pipe._execution_device
     generator = torch.Generator(device=device).manual_seed(seed)
     B, C, H, W = imgs.shape
+    lo, hi = shard_frames(B, shard)
     ctrl = frescoProc.controller
     ctrl.disable_controller()
     disable_FRESCO_opt(pipe)
     ctrl.clear_store()
     ctrl.enable_store()
     latents = pipe.prepare_latents(B, pipe.unet.config.in_channels, H, W, prompt_embeds.dtype, device, generator,
-                                   latents=None)
-    latent_x0 = pipe.vae.config.scaling_factor * pipe.vae.encode(imgs.to(pipe.unet.dtype)).latent_dist.sample()
+                                   latents=None)[lo:hi]             # all N frames: same Philox stream on every rank
+    latent_x0 = pipe.vae.config.scaling_factor * pipe.vae.encode(imgs[lo:hi].to(pipe.unet.dtype)).latent_dist.sample()
     latents = scheduler.add_noise(latent_x0, latents, timestep).detach()
+    chunks = 2 if do_classifier_free_guidance else 1
     model_in = torch.cat([latents] * 2) if do_classifier_free_guidance else latents
-    out = pipe.unet(model_in, timestep, encoder_hidden_states=prompt_embeds, cross_attention_kwargs=None,
-                    return_dict=False)
+    out = pipe.unet(model_in, timestep, encoder_hidden_states=chunk_frames(prompt_embeds, chunks, B, lo, hi),
+                    cross_attention_kwargs=None, return_dict=False)
     ctrl.disable_store()
     return gram_targets(out[1:])
 
 
 @torch.no_grad()
-def get_flow_and_interframe_paras(flow_model, imgs, visualize_pipeline=False):
+def get_flow_and_interframe_paras(flow_model, imgs, visualize_pipeline=False, shard=None):
     """Parameters for temporal-guided attention / optimisation (src/diffusion_hacked.py:905-957): bidirectional
     GMFlow flow between consecutive keyframes (incl. the wrap-around pair), occlusion masks from flow consistency
     and photometric error, the cross-frame K/V masks at 3 scales and the FLATTEN trajectories at 2 scales.
     ``imgs``: list of HxWx3 uint8 arrays.  ``flow_model``: a GMFlow instance (its global correlation can be
-    redirected to fresco_b200.gmflow_matching, see INTEGRATION.md)."""
+    redirected to fresco_b200.gmflow_matching, see INTEGRATION.md).
+
+    ``shard=(world, rank[, group])`` (not in the reference): every rank gets all N frames, runs GMFlow on its own
+    pairs [rank*N/G, (rank+1)*N/G) only and one all-gather assembles the whole batch's flows (rank order == pair
+    order).  Occlusions, masks and trajectories are then built from the gathered flows on every rank, as unsharded:
+    the return values are the whole batch's, as in the unsharded call."""
+    from .dist import all_gather_blocks, shard_frames
     from .flow_utils import flow_warp, forward_backward_consistency_check, get_mapping_ind
     dev = next(flow_model.parameters()).device
     images = torch.stack([torch.from_numpy(im).permute(2, 0, 1).float() for im in imgs], dim=0).to(dev)
     imgs_torch = images / 127.5 - 1.0                                   # numpy2tensor (src/utils.py:8-12)
     reshuffle = list(range(1, len(images))) + [0]
-    res = flow_model(images, images[reshuffle], attn_splits_list=[2], corr_radius_list=[-1], prop_radius_list=[-1],
-                     pred_bidir_flow=True)
-    fwd_flows, bwd_flows = res["flow_preds"][-1].chunk(2)
+    lo, hi = shard_frames(len(images), shard)
+    res = flow_model(images[lo:hi], images[reshuffle][lo:hi], attn_splits_list=[2], corr_radius_list=[-1],
+                     prop_radius_list=[-1], pred_bidir_flow=True)
+    flow = res["flow_preds"][-1]                                        # [2 * pairs, 2, H, W]: forward | backward
+    if shard is not None and shard[0] > 1:
+        world = shard[0]
+        gathered = all_gather_blocks(flow, world, shard[2] if len(shard) > 2 else None)
+        flow = gathered.view(world, 2, hi - lo, *flow.shape[1:]).transpose(0, 1).reshape(2 * len(images), *flow.shape[1:])
+    fwd_flows, bwd_flows = flow.chunk(2)
     fwd_flows, bwd_flows = fwd_flows.contiguous(), bwd_flows.contiguous()
     fwd_occs, bwd_occs = forward_backward_consistency_check(fwd_flows, bwd_flows)
     warped1 = flow_warp(images, bwd_flows)

@@ -37,6 +37,28 @@ def frame_range(n_frames: int, world: int, rank: int) -> Tuple[int, int]:
     return rank * per, (rank + 1) * per
 
 
+def shard_frames(n_frames: int, shard) -> Tuple[int, int]:
+    """frame range [lo, hi) of this rank for ``shard=(world, rank[, group])``; the whole batch for ``shard=None``"""
+    return (0, n_frames) if shard is None else frame_range(n_frames, shard[0], shard[1])
+
+
+def chunk_frames(t: Optional[torch.Tensor], chunks: int, n_frames: int, lo: int, hi: int) -> Optional[torch.Tensor]:
+    """Frames [lo, hi) of each CFG chunk of a ``(chunk, frame)``-major batch ``[chunks * n_frames, ...]`` (prompt
+    embeddings, ControlNet edges).  Anything not laid out that way (None, one prompt shared by all frames) and the
+    whole range come back as they are."""
+    if t is None or t.shape[0] != chunks * n_frames or hi - lo == n_frames:
+        return t
+    return t.view(chunks, n_frames, *t.shape[1:])[:, lo:hi].reshape(chunks * (hi - lo), *t.shape[1:])
+
+
+def all_gather_blocks(t: torch.Tensor, world: int, group=None) -> torch.Tensor:
+    """``[world, *t.shape]``: every rank's ``t`` in rank order (one all-gather)"""
+    t = t.contiguous()
+    out = torch.empty((world,) + tuple(t.shape), dtype=t.dtype, device=t.device)
+    dist.all_gather_into_tensor(out.view(-1, *t.shape[1:]), t, group=group)
+    return out
+
+
 class RingComm:
     """Neighbour exchange of the frame ring (SURVEY 8e, exchange 3): ``shift(send, recv, +1)`` sends ``send`` to rank+1
     and fills ``recv`` from rank-1 (``-1``: the other way round).  One batched NCCL send/recv pair on the current

@@ -108,7 +108,9 @@ def warp_tensor(sample, flows, occs, saliency, unet_chunk_size, shard=None):
     batch (flows / occs / saliency describe ALL N frames).  The chain is sequential over frames but independent per
     (chunk, channel) plane, so the batch is re-sharded by CHANNEL for the chain: one all-to-all turns
     [frames/G, all channels] into [all frames, channels/G], every rank runs the chain kernel on its channel slice, a
-    second all-to-all brings the frames back (SURVEY 8e, "sequential pieces")."""
+    second all-to-all brings the frames back (SURVEY 8e, "sequential pieces").  When the channels do not split over the
+    ranks (a decoded image has 3: background smoothing, src/pipe_FRESCO.py:46) every rank all-gathers the frames instead,
+    runs the chain on the whole batch and keeps its own frames."""
     world = 1 if shard is None else shard[0]
     n = sample.shape[0] // unet_chunk_size * world
     h, w = sample.shape[2], sample.shape[3]
@@ -133,19 +135,29 @@ def warp_tensor(sample, flows, occs, saliency, unet_chunk_size, shard=None):
     def chain(planes, chunks):
         return ops.warp_fuse_chain(planes, bwd_flow, fwd_flow_last, blend, chunks)
 
-    x = sample.contiguous()
-    # the shared-memory chain kernel takes fp16 or fp32 planes up to 100 KB; image-resolution planes (background
-    # smoothing, src/pipe_FRESCO.py:46, fp16 VAE output) run the per-step kernel, which works on fp32 like the
-    # reference's own `.to(torch.float32)` copy (flow_utils.py:36)
-    if x.dtype not in (torch.float16, torch.float32) or 2 * h * w * 4 > 200 * 1024:
-        x = x.float()
+    def chain_input(t):
+        # the shared-memory chain kernel takes fp16 or fp32 planes up to 100 KB; image-resolution planes (background
+        # smoothing, src/pipe_FRESCO.py:46, fp16 VAE output) run the per-step kernel, which works on fp32 like the
+        # reference's own `.to(torch.float32)` copy (flow_utils.py:36)
+        if t.dtype not in (torch.float16, torch.float32) or 2 * h * w * 4 > 200 * 1024:
+            return t.float()
+        return t
+
     if world == 1:
-        return chain(x, unet_chunk_size).to(sample.dtype)
+        return chain(chain_input(sample.contiguous()), unet_chunk_size).to(sample.dtype)
     import torch.distributed as dist
+    from .dist import all_gather_blocks
     group = shard[2] if len(shard) > 2 else None
-    chunks, n_local, C = unet_chunk_size, n // world, x.shape[1]
+    chunks, n_local, C = unet_chunk_size, n // world, sample.shape[1]
     if C % world != 0:
-        raise ValueError(f"{C} channels do not split evenly over {world} ranks")
+        # gather path: the frames travel in the dtype of ``sample`` (fp16 VAE output: 1.5 MB per 512^2 frame), the chain
+        # runs on exactly the batch the unsharded call sees
+        full = all_gather_blocks(sample, world, group)                               # [rank, chunk, frame, C, h, w]
+        full = full.view(world, chunks, n_local, C, h, w).transpose(0, 1).reshape(chunks * n, C, h, w)
+        fused = chain(chain_input(full), chunks).view(chunks, n, C, h, w)
+        lo = shard[1] * n_local
+        return fused[:, lo:lo + n_local].reshape(chunks * n_local, C, h, w).to(sample.dtype)
+    x = chain_input(sample.contiguous())
     cg = C // world
     send = x.view(chunks, n_local, world, cg, h * w).permute(2, 1, 0, 3, 4).contiguous()      # [dest, frame, chunk, cg, hw]
     recv = torch.empty_like(send)

@@ -10,7 +10,8 @@ Same names, arguments and behaviour.  What changes underneath:
   for ALL N frames from identically seeded generators on every rank and sliced, so the sample paths are those of the
   unsharded run (``repeat_noise`` needs frame 0's noise everywhere, :67-68, :150-151); ``record_latents`` (frames 0
   and N-1, :175-179) is assembled with one tiny all-gather per step; restoring frames 0-1 in propagation mode touches
-  rank 0 (and rank 1 when a rank holds a single frame).
+  rank 0 (and rank 1 when a rank holds a single frame); the background-smoothing steps decode, warp and re-encode only
+  this rank's frames (``warp_tensor(shard=...)`` gathers the decoded frames for the image-resolution chain).
 The VAE, ControlNet, scheduler tables and the UNet body stay what the caller passes in (diffusers objects or the bench
 harness).
 """
@@ -21,6 +22,7 @@ from typing import List, Optional
 import torch
 
 from . import ops
+from .dist import chunk_frames, shard_frames
 from .flow_utils import warp_tensor
 
 
@@ -41,12 +43,16 @@ def _step_coefficients(scheduler, timestep):
 
 
 def step(pipe, model_output, timestep, sample, generator, repeat_noise=False, visualize_pipeline=False, flows=None,
-         occs=None, saliency=None, guidance_scale: Optional[float] = None, noise: Optional[torch.Tensor] = None):
+         occs=None, saliency=None, guidance_scale: Optional[float] = None, noise: Optional[torch.Tensor] = None,
+         shard=None):
     """DDPM step with background smoothing (src/pipe_FRESCO.py:14-77).
 
     ``model_output`` is the guided noise prediction [N, ...] as in the reference; if ``guidance_scale`` is given it is
     the raw UNet output [2N, ...] (uncond | text) and the guidance (:212-215) is fused into the first kernel.
-    ``noise`` (optional) replaces the ``torch.randn`` draw of :61-62 (the frame-sharded loop passes its slice)."""
+    ``noise`` (optional) replaces the ``torch.randn`` draw of :61-62 (the frame-sharded loop passes its slice).
+    ``shard=(world, rank[, group])``: ``sample`` holds this rank's frames of a frame-sharded batch (``flows`` / ``occs``
+    / ``saliency`` the whole batch's); background smoothing decodes and re-encodes those frames only and warps them
+    along the whole chain."""
     alpha_prod_t, c_x0, c_xt, sigma = _step_coefficients(pipe.scheduler, timestep)
     sample = sample.contiguous()
     do_cfg = guidance_scale is not None
@@ -54,22 +60,13 @@ def step(pipe, model_output, timestep, sample, generator, repeat_noise=False, vi
                                            alpha_prod_t, do_cfg=do_cfg)
     if saliency is not None and flows is not None and occs is not None:                        # :44-47
         image = pipe.vae.decode(pred_original_sample / pipe.vae.config.scaling_factor).sample
-        image = warp_tensor(image, flows, occs, saliency, unet_chunk_size=1)
+        image = warp_tensor(image, flows, occs, saliency, unet_chunk_size=1, shard=shard)
         pred_original_sample = (pipe.vae.config.scaling_factor * pipe.vae.encode(image).latent_dist.sample()).contiguous()
     if noise is None:
         noise = torch.randn(sample.shape, generator=generator, device=sample.device, dtype=sample.dtype)
     pred_prev_sample = ops.ddpm_prev(pred_original_sample, sample, noise.contiguous(), c_x0, c_xt, sigma,
                                      repeat_noise=repeat_noise)
     return (pred_prev_sample, pred_original_sample)
-
-
-def _frame_slice(n: int, shard):
-    if shard is None:
-        return 0, n
-    world, rank = shard[0], shard[1]
-    if n % world != 0:
-        raise ValueError(f"{n} frames do not split evenly over {world} ranks")
-    return rank * (n // world), (rank + 1) * (n // world)
 
 
 def _gather_first_last(latents_local, n, lo, hi, shard):
@@ -92,13 +89,14 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
               bg_smoothing_steps=[16, 17], shard=None):
     """Video-to-video translation of one keyframe batch with FRESCO (src/pipe_FRESCO.py:81-234).
 
-    ``imgs`` / ``edges`` / ``prompt_embeds`` hold ALL N frames (every rank gets the same arguments); with
-    ``shard=(world, rank[, group])`` this rank denoises frames [rank*N/G, (rank+1)*N/G) and returns their latents."""
+    ``imgs`` / ``edges`` / ``prompt_embeds`` / ``flows`` / ``occs`` / ``saliency`` hold ALL N frames (every rank gets the
+    same arguments); with ``shard=(world, rank[, group])`` this rank denoises frames [rank*N/G, (rank+1)*N/G) and
+    returns their latents, the background-smoothing steps included."""
     device = pipe._execution_device
     noise_scheduler = pipe.scheduler
     generator = torch.Generator(device=device).manual_seed(seed)
     B, C, H, W = imgs.shape
-    lo, hi = _frame_slice(B, shard)
+    lo, hi = shard_frames(B, shard)
     latents = pipe.prepare_latents(B, pipe.unet.config.in_channels, H, W, prompt_embeds.dtype, device, generator,
                                    latents=None)                                # all N frames: same Philox stream everywhere
     if repeat_noise:
@@ -111,10 +109,7 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
         latents_init = noise_scheduler.add_noise(latent_x0, latents[lo:hi], timesteps[num_warmup_steps]).detach()
     n_local = hi - lo
     chunks = 2 if do_classifier_free_guidance else 1
-    if prompt_embeds.shape[0] == chunks * B and n_local != B:                  # (b f) layout: slice the frames of each chunk
-        pe = prompt_embeds.view(chunks, B, *prompt_embeds.shape[1:])[:, lo:hi].reshape(chunks * n_local, *prompt_embeds.shape[1:])
-    else:
-        pe = prompt_embeds
+    pe = chunk_frames(prompt_embeds, chunks, B, lo, hi)                       # (b f) layout: the frames of each chunk
     sub_flows = sub_occs = sub_sal = None
     latents = latents_init
     for i, t in enumerate(timesteps[num_warmup_steps:]):
@@ -132,9 +127,7 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
             record_latents += [_gather_first_last(latents, B, lo, hi, shard)]
         latent_model_input = torch.cat([latents] * 2) if do_classifier_free_guidance else latents
         if use_controlnet:
-            e = edges
-            if e is not None and e.shape[0] == chunks * B and n_local != B:
-                e = e.view(chunks, B, *e.shape[1:])[:, lo:hi].reshape(chunks * n_local, *e.shape[1:])
+            e = chunk_frames(edges, chunks, B, lo, hi)
             down_block_res_samples, mid_block_res_sample = controlnet(
                 latent_model_input, t, encoder_hidden_states=pe, controlnet_cond=e,
                 conditioning_scale=cond_scale[i + num_warmup_steps], guess_mode=False, return_dict=False)
@@ -148,10 +141,7 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
                                  dtype=latents.dtype)
         noise = full_noise[0:1].expand(n_local, *latents.shape[1:]).contiguous() if repeat_noise else full_noise[lo:hi]
         smooth = (i + num_warmup_steps) in bg_smoothing_steps
-        if smooth and shard is not None:
-            raise NotImplementedError("background smoothing warps along the frame chain: run those steps unsharded "
-                                      "(all-gather the latents) -- see DESIGN.md, multi-GPU")
         latents = step(pipe, noise_pred, t, latents, generator, visualize_pipeline=visualize_pipeline,
                        flows=flows if smooth else None, occs=occs if smooth else None, saliency=saliency if smooth else None,
-                       guidance_scale=guidance_scale if do_classifier_free_guidance else None, noise=noise)[0]
+                       guidance_scale=guidance_scale if do_classifier_free_guidance else None, noise=noise, shard=shard)[0]
     return latents
