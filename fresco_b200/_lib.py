@@ -21,6 +21,7 @@ _SIGNATURES = {
     "fresco_abi_version": (c_int, []),
     "fresco_last_error": (c_char_p, []),
     "fresco_launch_count": (c_longlong, []),
+    "fresco_last_kernel": (c_char_p, []),
     "fresco_set_option": (c_int, [c_char_p, c_int]),
     "fresco_attn_variant": (c_char_p, [c_int]),
     "fresco_kv_compact": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
@@ -113,3 +114,8 @@ def set_option(name: str, value: int) -> None:
 
 def launch_count() -> int:
     return int(lib().fresco_launch_count())
+
+
+def last_kernel() -> str:
+    """Name of the last kernel the library launched on this thread, template arguments included."""
+    return (lib().fresco_last_kernel() or b"").decode()

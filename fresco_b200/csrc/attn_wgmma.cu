@@ -312,6 +312,9 @@ static int make_head_tile_map(CUtensorMap* map, const void* base, int head_dim, 
   return rc;
 }
 
+// launch name of a variant; fresco_attn_variant reports the same string
+#define ATTN_NAME_FMT "fresco_attn_kernel<%d,keys%d,wg%d,poly%d%s>"
+
 template <int D, int KN, int NWG, int POLY, bool ROWSUM>
 static int launch_variant(const void* q, const void* k, const void* v, void* out, int batch_q, int q_len, int kv_len,
                           int heads, int q_per_kv, long long kv_row_stride, long long kv_batch_stride,
@@ -332,7 +335,7 @@ static int launch_variant(const void* q, const void* k, const void* v, void* out
   }
   dim3 grid((q_len + Cfg::TILE_M - 1) / Cfg::TILE_M, heads, batch_q);
   fresco_attn_kernel<D, KN, NWG, POLY, ROWSUM><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(tq, tk, tv, p);
-  return check_launch("fresco_attn_kernel");
+  return check_launchf(ATTN_NAME_FMT, D, KN, NWG, POLY, ROWSUM ? ",rowsum" : "");
 }
 
 // the variant the options select for a head dim (see the comment at the top of this file)
@@ -394,8 +397,9 @@ using namespace fresco;
 extern "C" const char* fresco_attn_variant(int head_dim) {
   static thread_local char buf[96];
   const AttnVariant a = attn_variant(head_dim);
-  snprintf(buf, sizeof(buf), "fresco_attn_kernel<%d,keys%d,wg%d,poly%d%s> (wgmma)", head_dim, a.wide == 0 ? 64 : 128,
-           a.wide == 2 ? 3 : 2, a.poly, a.rowsum ? ",rowsum" : "");
+  const int n = snprintf(buf, sizeof(buf), ATTN_NAME_FMT, head_dim, a.wide == 0 ? 64 : 128, a.wide == 2 ? 3 : 2, a.poly,
+                         a.rowsum ? ",rowsum" : "");
+  snprintf(buf + n, sizeof(buf) - n, " (wgmma)");
   return buf;
 }
 

@@ -10,7 +10,10 @@ namespace fresco {
 
 int set_error(int code, const char* msg);
 int set_cuda_error(cudaError_t e, const char* where);
+// records `kernel` as the calling thread's last launch (fresco_last_kernel) and checks the launch for errors;
+// check_launchf formats the name, so a templated launch site can name its instantiation
 int check_launch(const char* kernel);
+int check_launchf(const char* fmt, ...) __attribute__((format(printf, 1, 2)));
 
 // cuTensorMapEncodeTiled resolved at run time through cudaGetDriverEntryPoint, so the library
 // has no link-time dependency on libcuda.so (it must load on a driver-less build box).

@@ -239,7 +239,8 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmP
     attr_set = true;
   }
   tile_gemm_kernel<EPI, B_MN><<<grid, kGThreads, kGSmem, s>>>(ta, tb, p);
-  return check_launch("tile_gemm_kernel");
+  static const char* const kEpiNames[] = {"EPI_STORE", "EPI_GRAM_SIGN", "EPI_GMFLOW"};
+  return check_launchf("tile_gemm_kernel<%s,%d>", kEpiNames[EPI], (int)B_MN);
 }
 
 // ghat [batch, L, C] fp32 (token-major)  ->  grad [batch, C, L] += (ghat - (ghat . xhat) xhat) / norm

@@ -229,7 +229,7 @@ static int launch_gram2(const CUtensorMap& a0, const CUtensorMap& b0, const CUte
   int grid = sm_count();
   if (grid > p.n_tiles) grid = p.n_tiles;
   gram2_kernel<MODE><<<grid, kG2Threads, kG2Smem, s>>>(a0, b0, a1, b1, p);
-  return check_launch("gram2_kernel");
+  return check_launch(MODE == G2_SIGN ? "gram2_kernel<G2_SIGN>" : "gram2_kernel<G2_GRAD>");
 }
 
 }  // namespace fresco

@@ -1546,7 +1546,7 @@ static int launch_temporal_rows(const void* q_raw, const void* k_raw, const void
   temporal_attn_rows_kernel<D, NMAX><<<blocks, threads, smem, s>>>(
       (const __half*)q_raw, (const __half*)k_raw, (const __half*)v_src, (__half*)out, fwd_map, traj_mask, frames, tokens,
       heads, tpb, scale * 1.4426950408889634f, in_row_stride / 8);
-  return check_launch("temporal_attn_rows_kernel");
+  return check_launchf("temporal_attn_rows_kernel<%d,%d>", D, NMAX);
 }
 
 extern "C" int fresco_temporal_attn_fwd(const void* q_raw, const void* k_raw, const void* v_src, void* out,
@@ -1622,7 +1622,7 @@ static int launch_chain_group(const void* sample, void* out, const float* bwd_fl
   const int planes = chunks * channels;
   warp_chain_group_kernel<T, K><<<(planes + K - 1) / K, 512, smem, s>>>((const T*)sample, (T*)out, bwd_flow, fwd_flow_last,
                                                                        blend, frames, channels, planes, h, w);
-  return check_launch("warp_chain_group_kernel");
+  return check_launchf("warp_chain_group_kernel<%s,%d>", sizeof(T) == 2 ? "half" : "float", K);
 }
 
 // (P pixels per thread, NQ channel quads per CTA) for a plane of hw pixels: as many quads as shared memory (bytes_per_px
@@ -1660,7 +1660,7 @@ static int launch_chain_quad(const void* sample, void* out, const float* bwd_flo
   }
   warp_chain_quad_kernel<T, P, NQ><<<chunks * channels / (4 * NQ), threads, smem, s>>>(
       (const T*)sample, (T*)out, bwd_flow, fwd_flow_last, blend, frames, channels, h, w);
-  return check_launch("warp_chain_quad_kernel");
+  return check_launchf("warp_chain_quad_kernel<%s,%d,%d>", sizeof(T) == 2 ? "half" : "float", P, NQ);
 }
 
 template <typename T>
@@ -1773,7 +1773,7 @@ extern "C" int fresco_warp_loss_fwd_bwd_halo(const float* cs, const float* fwd_f
     warp_loss_quad_kernel<PP, QQ><<<grid_q, threads, smem_q, s>>>(                                                      \
         cs, fwd_flow, bwd_flow, fwd_keep, bwd_keep, (const uint4*)bwd_ell, (const uint4*)fwd_ell, overflow, n_overflow, \
         grad, loss_acc, accumulate, frames, channels, h, w, kk, halo_cs, halo_grad);                                    \
-    return check_launch("warp_loss_quad_kernel");                                                                       \
+    return check_launchf("warp_loss_quad_kernel<%d,%d>", PP, QQ);                                                       \
   }
       LQ(1, 4) LQ(2, 2) LQ(4, 1) LQ(1, 2) LQ(2, 1) LQ(1, 1)
 #undef LQ
@@ -1811,7 +1811,7 @@ extern "C" int fresco_warp_loss_fwd_bwd_halo(const float* cs, const float* fwd_f
                                                          (const uint4*)bwd_ell, (const uint4*)fwd_ell, overflow,        \
                                                          n_overflow, grad, loss_acc, accumulate, frames, channels,      \
                                                          planes, h, w, G, kk, halo_cs, halo_grad);                      \
-    rc = check_launch("warp_loss_group_kernel");                                                                        \
+    rc = check_launchf("warp_loss_group_kernel<%d,%d>", PP, KK);                                                        \
   }
       LOSS_CASE(1, 1) LOSS_CASE(1, 2) LOSS_CASE(1, 4)
       LOSS_CASE(2, 1) LOSS_CASE(2, 2) LOSS_CASE(2, 4)
@@ -1868,7 +1868,7 @@ extern "C" int fresco_adain(const float* content, const void* style, void* out, 
     adain_kernel<__half><<<planes, 256, 0, (cudaStream_t)stream>>>(content, (const __half*)style, (__half*)out, hw, 1);
   else
     adain_kernel<float><<<planes, 256, 0, (cudaStream_t)stream>>>(content, (const float*)style, (float*)out, hw, 0);
-  return check_launch("adain_kernel");
+  return check_launch(is_half ? "adain_kernel<half>" : "adain_kernel<float>");
 }
 
 extern "C" int fresco_gram_normalize(const float* cs, void* xhat, float* norms, int batch, int channels, int tokens,
@@ -1893,7 +1893,7 @@ extern "C" int fresco_cfg_pred_x0(const void* noise_uncond, const void* noise_te
   else
     cfg_pred_x0_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>((const float*)noise_uncond, (const float*)noise_text,
                                                                       (const float*)sample, (float*)x0, n, guidance_scale, sb, isa);
-  return check_launch("cfg_pred_x0_kernel");
+  return check_launch(is_half ? "cfg_pred_x0_kernel<half>" : "cfg_pred_x0_kernel<float>");
 }
 
 extern "C" int fresco_ddpm_prev(const void* x0, const void* sample, const void* noise, void* prev, int is_half, long long n,
@@ -1907,7 +1907,7 @@ extern "C" int fresco_ddpm_prev(const void* x0, const void* sample, const void* 
   else
     ddpm_prev_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>((const float*)x0, (const float*)sample, (const float*)noise,
                                                                     (float*)prev, n, per_frame, repeat_noise, c_x0, c_xt, sigma);
-  return check_launch("ddpm_prev_kernel");
+  return check_launch(is_half ? "ddpm_prev_kernel<half>" : "ddpm_prev_kernel<float>");
 }
 
 extern "C" int fresco_dilate(const float* in, float* out, int planes, int h, int w, int kernel, void* stream) {

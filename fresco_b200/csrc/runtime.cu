@@ -1,5 +1,6 @@
 // Error state, launch accounting and the driver-API entry point for TMA tensor maps.
 #include <atomic>
+#include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -10,6 +11,7 @@ namespace fresco {
 
 static thread_local char g_err[512] = "";
 static std::atomic<long long> g_launches{0};
+static thread_local char g_last_kernel[128] = "";
 
 int set_error(int code, const char* msg) {
   snprintf(g_err, sizeof(g_err), "%s", msg);
@@ -23,9 +25,19 @@ int set_cuda_error(cudaError_t e, const char* where) {
 
 int check_launch(const char* kernel) {
   g_launches.fetch_add(1, std::memory_order_relaxed);
+  snprintf(g_last_kernel, sizeof(g_last_kernel), "%s", kernel);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_cuda_error(e, kernel);
   return FRESCO_OK;
+}
+
+int check_launchf(const char* fmt, ...) {
+  char name[sizeof(g_last_kernel)];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(name, sizeof(name), fmt, ap);
+  va_end(ap);
+  return check_launch(name);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -97,6 +109,7 @@ int sm_count() {
 extern "C" int fresco_abi_version(void) { return FRESCO_ABI_VERSION; }
 extern "C" const char* fresco_last_error(void) { return fresco::g_err; }
 extern "C" long long fresco_launch_count(void) { return fresco::g_launches.load(); }
+extern "C" const char* fresco_last_kernel(void) { return fresco::g_last_kernel; }
 extern "C" int fresco_set_option(const char* name, int value) {
   using namespace fresco;
   if (!name) return set_error(FRESCO_ERR_ARG, "fresco_set_option: null name");

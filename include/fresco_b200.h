@@ -35,6 +35,9 @@ int fresco_abi_version(void);
 const char* fresco_last_error(void);
 /* number of kernels launched by this library in this process (for bench.py's gpu_launches) */
 long long fresco_launch_count(void);
+/* name of the last kernel this library launched on the calling thread, with its template arguments where the launch
+ * site picks an instantiation (e.g. "warp_loss_group_kernel<18,1>"); "" before the first launch (thread-local string) */
+const char* fresco_last_kernel(void);
 /* tuning option by the name of its environment variable (FRESCO_ATTN_WIDE, FRESCO_ATTN_POLY, FRESCO_ATTN_ROWSUM,
  * FRESCO_TEMPORAL_V, FRESCO_GRAM_V); the environment is read once, this overrides it;
  * value < 0 restores the built-in default. */

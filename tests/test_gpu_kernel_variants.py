@@ -1,0 +1,655 @@
+"""Every kernel instantiation the launchers can select, at the shapes that select it, against fp64 references.
+
+The launchers in hbm_kernels.cu, gemm_wgmma.cu, gram_wgmma.cu and attn_wgmma.cu pick a template instantiation from
+the frame count, the head dim, the plane size measured against shared memory, the channel divisibility, the SM count,
+whether the input rows are strided, and the tuning options.  The file is one table, ``ROWS``: an entry point, a shape,
+the options, and the kernels the call must launch, in order, as ``fresco_last_kernel()`` names them.  Each row
+
+* fills every output with NaN (or a NaN bit pattern) first, so a row or tile the kernel never writes is caught,
+* runs the entry point through the C ABI and asserts the instantiation it launched -- a change to a selection rule
+  fails here instead of quietly moving a row to another kernel,
+* compares the output with a plain fp64 reference of the same operation, evaluated on the operands the kernel consumes
+  (fp16-rounded where the kernel reads fp16).  The temporal-consistency loss keeps the fp32 oracle and tolerance of
+  ``test_temporal_loss_teacher_forced_layer_shapes``.
+
+Instantiations no row reaches are listed with the reason in ``UNREACHABLE`` (no shape or SM count selects them),
+``NOT_LAST`` (launched, but another kernel of the same call is what the record shows) or ``COVERED_ELSEWHERE``
+(one instantiation per dtype, no selection; the named test checks it).  ``test_launch_name_universe`` derives the
+instantiation lists from the launcher sources and checks that every name is in exactly one of those places.
+"""
+import collections
+import functools
+import math
+import os
+import re
+
+import pytest
+import torch
+import torch.nn.functional as F
+
+from oracle import fresco_oracle as O
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+CSRC = os.path.join(ROOT, "fresco_b200", "csrc")
+
+
+@pytest.fixture(scope="module")
+def fb():
+    if not torch.cuda.is_available():
+        pytest.skip("GPU tests need a CUDA device")
+    from fresco_b200 import _lib, ops
+    _lib.lib()      # fails loudly if the extension is missing
+    torch.backends.cuda.matmul.allow_tf32 = False
+    torch.backends.cudnn.allow_tf32 = False
+
+    class NS:
+        pass
+    ns = NS()
+    ns.lib, ns.ops, ns.c = _lib, ops, _lib.lib()
+    return ns
+
+
+def P(t):
+    return t.data_ptr()
+
+
+class Launches:
+    """Checks each launch of a row against the table as it happens."""
+
+    def __init__(self, fb, row):
+        self.fb, self.row, self.i = fb, row, 0
+
+    def __call__(self, what, rc=0):
+        self.fb.lib.check(rc, what)
+        name = self.fb.lib.last_kernel()
+        assert self.i < len(self.row.kernels), f"{what}: unexpected launch of {name}"
+        want = self.row.kernels[self.i]
+        self.i += 1
+        assert name == want, f"{what} launched {name}; the table expects {want}"
+        SEEN.add(name)
+
+
+Row = collections.namedtuple("Row", "id kernels run opts")
+ROWS = []
+SEEN = set()
+RAN = set()
+
+
+def row(id_, kernels, fn, opts=None, **kw):
+    ROWS.append(Row(id_, tuple(kernels), functools.partial(fn, **kw), dict(opts or {})))
+
+
+def _nan(shape, dtype):
+    return torch.full(shape, float("nan"), dtype=dtype, device="cuda")
+
+
+def _check_close(out, ref, bound, what):
+    """max |out - ref| <= bound over every element; NaN left in ``out`` (never written) fails."""
+    out = out.double()
+    unwritten = (~torch.isfinite(out)).sum().item()
+    assert unwritten == 0, f"{what}: {unwritten} outputs not written (NaN) or not finite"
+    err = (out - ref).abs().max().item()
+    assert err <= bound, f"{what}: max error {err:.3g} > {bound:.3g}"
+
+
+def _worst_tile(ratio, rows=128, cols=256):
+    """Where err / tol is largest, by rows x cols output tile (ratio [R, C]; NaN counts as infinitely wrong)."""
+    ratio = torch.nan_to_num(ratio.double(), nan=float("inf"))
+    R, C = ratio.shape
+    t = F.pad(ratio, (0, (-C) % cols, 0, (-R) % rows)).view((R + rows - 1) // rows, rows, (C + cols - 1) // cols, cols)
+    t = t.amax((1, 3))
+    i, j = divmod(int(t.argmax().item()), t.shape[1])
+    return (f"worst {rows}x{cols} tile rows [{i * rows}, {(i + 1) * rows}) cols [{j * cols}, {(j + 1) * cols}): "
+            f"max err/tol {t[i, j].item():.3g}; {(t > 1).sum().item()} of {t.numel()} tiles fail")
+
+
+# ================================================================================================ temporal attention
+def _trajectories(N, L, seed):
+    """Random per-frame permutations and masks with the reference's structure (cuts between frames <= i and > i,
+    flow_utils.py:126-133), plus 5 % of trajectories where a frame may only attend to itself."""
+    g = torch.Generator().manual_seed(seed)
+    fwd = torch.stack([torch.arange(L)] + [torch.randperm(L, generator=g) for _ in range(N - 1)])
+    mask = torch.ones(L, N, N, dtype=torch.bool)
+    for i in range(N - 1):
+        cut = torch.ones(N, N, dtype=torch.bool)
+        cut[:i + 1, i + 1:] = False
+        cut[i + 1:, :i + 1] = False
+        sel = torch.rand(L, generator=g) < 0.15
+        mask[sel] = mask[sel] & cut
+    mask[torch.rand(L, generator=g) < 0.05] = torch.eye(N, dtype=torch.bool)
+    return fwd, mask
+
+
+def _temporal_ref(q, k, v, fwd, mask, chunks, heads, scale):
+    """fp64: out[b, f, fwd[f, p]] = softmax_g(q[f, .] . k[g, .] * scale, masked) v[g, .] along trajectory p."""
+    B, L, C = q.shape
+    N, d = B // chunks, C // heads
+    pos = fwd.cuda()
+    fr = torch.arange(N, device="cuda")[:, None]
+    m = mask.cuda()[:, None]
+    out = torch.empty(B, L, C, dtype=torch.float64, device="cuda")
+    for b in range(chunks):
+        sl = slice(b * N, (b + 1) * N)
+        qb, kb, vb = (t[sl][fr, pos].double().reshape(N, L, heads, d) for t in (q, k, v))
+        s = torch.einsum("flhd,glhd->lhfg", qb, kb) * scale
+        p = torch.softmax(s.masked_fill(~m, float("-inf")), -1)
+        ob = out[sl]
+        ob[fr, pos] = torch.einsum("lhfg,glhd->flhd", p, vb).reshape(N, L, C)
+    return out
+
+
+def _temporal(fb, launch, N, L, heads, d, packed=False, chunks=2, seed=0):
+    """packed=False: fresco_temporal_attn_fwd on dense [chunks*N, L, C] tensors.  packed=True: the call
+    ShardedTrajectoryExchange.run makes -- qkv [N, chunks*L, 3C] with q | k | v in every row, identity map, chunks=1,
+    mask [chunks*L, N, N] (L = this rank's trajectories)."""
+    C, scale = heads * d, 1.0 / math.sqrt(d)
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    fwd, mask = _trajectories(N, L, seed)
+    if packed:
+        tokens = chunks * L
+        qkv = torch.randn(N, tokens, 3 * C, device="cuda", generator=g)
+        qkv[..., C:2 * C] *= 2.0
+        qkv = qkv.half()
+        q, k, v = qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:]
+        pq, pk, pv = P(qkv), P(qkv) + 2 * C, P(qkv) + 4 * C
+        fwd = torch.arange(tokens)[None].expand(N, -1).contiguous()
+        mask = mask[None].expand(chunks, -1, -1, -1).reshape(tokens, N, N)
+        kchunks, stride = 1, 3 * C
+    else:
+        tokens = L
+        q = torch.randn(chunks * N, L, C, device="cuda", generator=g).half()
+        k = (torch.randn(chunks * N, L, C, device="cuda", generator=g) * 2.0).half()
+        v = torch.randn(chunks * N, L, C, device="cuda", generator=g).half()
+        pq, pk, pv = P(q), P(k), P(v)
+        kchunks, stride = chunks, C
+    fwd_d, mask_d = fwd.cuda().contiguous(), mask.to(torch.uint8).cuda().contiguous()
+    out = _nan((kchunks * N, tokens, C), torch.float16)
+    launch("fresco_temporal_attn_fwd_strided",
+           fb.c.fresco_temporal_attn_fwd_strided(pq, pk, pv, P(out), P(fwd_d), P(mask_d), kchunks, N, tokens, heads, d,
+                                                 stride, scale, fb.lib.stream()))
+    ref = _temporal_ref(q, k, v, fwd, mask, kchunks, heads, scale)
+    # the stated fp16 attention bound, over every output row
+    _check_close(out, ref, 2e-3 * ref.abs().max().item(), "temporal attention")
+
+
+for _N, _d, _L in [(9, 40, 4096), (12, 40, 4096), (16, 40, 4096), (9, 80, 1024), (12, 80, 1024), (16, 80, 1024)]:
+    # N = 16, 8 heads: 128 rows per trajectory, so 2 trajectories per CTA at d = 40 and 1 at d = 80 (48 KB)
+    row(f"temporal-N{_N}-d{_d}", [f"temporal_attn_rows_kernel<{_d},16>"], _temporal, N=_N, L=_L, heads=8, d=_d)
+row("temporal-N8-d40", ["temporal_attn_rows_kernel<40,8>"], _temporal, N=8, L=4096, heads=8, d=40)
+row("temporal-N4-d80", ["temporal_attn_rows_kernel<80,8>"], _temporal, N=4, L=1024, heads=8, d=80)
+row("temporal-N5-d64", ["temporal_attn_rows_kernel<64,8>"], _temporal, N=5, L=500, heads=4, d=64)
+row("temporal-N13-d64", ["temporal_attn_rows_kernel<64,16>"], _temporal, N=13, L=500, heads=4, d=64)
+row("temporal-packed-N16-d40", ["temporal_attn_rows_kernel<40,16>"], _temporal, N=16, L=4096 // 2, heads=8, d=40,
+    packed=True)
+row("temporal-packed-N16-d80", ["temporal_attn_rows_kernel<80,16>"], _temporal, N=16, L=1024 // 2, heads=8, d=80,
+    packed=True)
+row("temporal-packed-N5-d64", ["temporal_attn_rows_kernel<64,8>"], _temporal, N=5, L=300, heads=4, d=64, packed=True)
+row("temporal-round1-N17-d40", ["temporal_attn_kernel"], _temporal, N=17, L=1024, heads=8, d=40)
+row("temporal-round1-N24-d80", ["temporal_attn_kernel"], _temporal, N=24, L=512, heads=8, d=80)
+row("temporal-round1-N4-d128", ["temporal_attn_kernel"], _temporal, N=4, L=300, heads=2, d=128)
+row("temporal-V1-N8-d40", ["temporal_attn_kernel"], _temporal, opts={"FRESCO_TEMPORAL_V": 1}, N=8, L=4096, heads=8,
+    d=40)
+
+
+# ================================================================================================ cross-frame attention
+def attn_name(d, wide, poly, rowsum):
+    keys = 64 if wide == 0 else 128
+    wg = 3 if wide == 2 and d <= 64 else 2
+    return "fresco_attn_kernel<%d,keys%d,wg%d,poly%d%s>" % (d, keys, wg, poly, ",rowsum" if wide == 0 and rowsum else "")
+
+
+def _attn_ref(q, k, v, heads, qpk, scale):
+    Bq, Lq, C = q.shape
+    d = C // heads
+    out = torch.empty(Bq, Lq, C, dtype=torch.float64, device="cuda")
+    for b in range(Bq):
+        qh = q[b].double().reshape(Lq, heads, d).transpose(0, 1)
+        kh = k[b // qpk].double().reshape(-1, heads, d).transpose(0, 1)
+        vh = v[b // qpk].double().reshape(-1, heads, d).transpose(0, 1)
+        out[b] = (torch.softmax(qh @ kh.transpose(1, 2) * scale, -1) @ vh).transpose(0, 1).reshape(Lq, C)
+    return out
+
+
+def _attn(fb, launch, d, qpk, Lq, Lk, heads=8, chunks=2, pad=0, gain=4.0, seed=0):
+    """fresco_attn_fwd_kv_strided as attn_fwd_kv_packed calls it: K | V side by side in one [chunks, Lk, 2C] buffer,
+    q_per_kv query frames per K/V batch.  pad > 0: batches (Lk + pad) rows apart, the pad rows NaN (a padded exchange
+    buffer); they must not reach the output."""
+    C, scale = heads * d, 1.0 / math.sqrt(d)
+    g = torch.Generator(device="cuda").manual_seed(seed + d + qpk)
+    q = (torch.randn(chunks * qpk, Lq, C, device="cuda", generator=g) * gain).half()
+    kv = torch.randn(chunks, Lk + pad, 2 * C, device="cuda", generator=g).half()
+    kv[:, Lk:] = float("nan")
+    out = _nan(q.shape, torch.float16)
+    launch("fresco_attn_fwd_kv_strided",
+           fb.c.fresco_attn_fwd_kv_strided(P(q), P(kv), P(kv) + 2 * C, P(out), chunks * qpk, Lq, Lk, heads, d, qpk, 2 * C,
+                                           (Lk + pad) * 2 * C, scale, 0.0, fb.lib.stream()))
+    assert fb.c.fresco_attn_variant(d).decode() == fb.lib.last_kernel() + " (wgmma)"
+    ref = _attn_ref(q, kv[:, :Lk, :C], kv[:, :Lk, C:], heads, qpk, scale)
+    _check_close(out, ref, 2e-3 * ref.abs().max().item(), "attention")
+
+
+for _d in (40, 80):
+    for _qpk in (2, 4, 8, 16):          # frame-sharded G = 8 / 4 / 2 (N_local query frames per K/V batch), unsharded N = 16
+        for _wide in (1, 0):
+            row(f"attn-kv-packed-d{_d}-qpk{_qpk}-wide{_wide}", [attn_name(_d, _wide, 0, 0)], _attn,
+                opts={"FRESCO_ATTN_WIDE": _wide}, d=_d, qpk=_qpk, Lq=1000, Lk=150 * _qpk + 37)
+    for _wide in (1, 0):
+        row(f"attn-kv-padded-d{_d}-wide{_wide}", [attn_name(_d, _wide, 0, 0)], _attn, opts={"FRESCO_ATTN_WIDE": _wide},
+            d=_d, qpk=4, Lq=700, Lk=613, pad=91)
+# every variant the options select, at every head dim (three consumer warpgroups stop at head dim 64)
+for _d in (40, 64, 80, 128):
+    for _wide in ((0, 1, 2) if _d <= 64 else (0, 1)):
+        for _poly in (0, 4, 8):
+            for _rowsum in ((0, 1) if _wide == 0 else (0,)):
+                row(f"attn-variant-d{_d}-wide{_wide}-poly{_poly}-rowsum{_rowsum}", [attn_name(_d, _wide, _poly, _rowsum)],
+                    _attn, opts={"FRESCO_ATTN_WIDE": _wide, "FRESCO_ATTN_POLY": _poly, "FRESCO_ATTN_ROWSUM": _rowsum},
+                    d=_d, qpk=2, Lq=300, Lk=1000, heads=2)
+
+
+# ================================================================================================ data movement
+def _bits(t):
+    return t.view(torch.int16)
+
+
+def _kv_compact_packed(fb, launch, chunks=2, N=4, tokens=500, C=320, extra=13):
+    g = torch.Generator(device="cuda").manual_seed(1)
+    k = torch.randn(chunks * N, tokens, C, device="cuda", generator=g).half()
+    v = torch.randn(chunks * N, tokens, C, device="cuda", generator=g).half()
+    idx = torch.nonzero(torch.rand(N * tokens, device="cuda", generator=g) < 0.4).reshape(-1).to(torch.int32)
+    n_sel = idx.numel()
+    kv = _nan((chunks, n_sel + extra, 2 * C), torch.float16)
+    launch("fresco_kv_compact_packed", fb.c.fresco_kv_compact_packed(P(k), P(v), P(idx), P(kv), chunks, N * tokens, n_sel,
+                                                                     n_sel + extra, C, fb.lib.stream()))
+    li = idx.long()
+    assert torch.equal(_bits(kv[:, :n_sel, :C]), _bits(k.reshape(chunks, N * tokens, C)[:, li]))
+    assert torch.equal(_bits(kv[:, :n_sel, C:]), _bits(v.reshape(chunks, N * tokens, C)[:, li]))
+    assert torch.equal(_bits(kv[:, n_sel:]), _bits(_nan((chunks, extra, 2 * C), torch.float16))), "rows past n_sel written"
+
+
+def _rows_gather(fb, launch, col, R=3000, n=2500, C=320):
+    g = torch.Generator(device="cuda").manual_seed(2 + col)
+    src = torch.randn(R, C, device="cuda", generator=g).half()
+    idx = torch.randint(0, R, (n,), device="cuda", generator=g, dtype=torch.int32)
+    dst = _nan((n, 3 * C), torch.float16)
+    launch("fresco_rows_gather", fb.c.fresco_rows_gather(P(src), P(idx), P(dst), n, C * 2, 3 * C * 2, col * C * 2,
+                                                         fb.lib.stream()))
+    want = _nan((n, 3 * C), torch.float16)
+    want[:, col * C:(col + 1) * C] = src[idx.long()]
+    assert torch.equal(_bits(dst), _bits(want))
+
+
+def _rows_scatter(fb, launch, R=3000, n=2500, C=320):
+    g = torch.Generator(device="cuda").manual_seed(3)
+    src = torch.randn(n, C, device="cuda", generator=g).half()
+    idx = torch.randperm(R, device="cuda", generator=g)[:n].to(torch.int32)
+    dst = _nan((R, C), torch.float16)
+    launch("fresco_rows_scatter", fb.c.fresco_rows_scatter(P(src), P(idx), P(dst), n, C * 2, fb.lib.stream()))
+    want = _nan((R, C), torch.float16)
+    want[idx.long()] = src
+    assert torch.equal(_bits(dst), _bits(want))
+
+
+row("kv-compact-packed-padded", ["kv_compact_packed_kernel"], _kv_compact_packed)
+for _col in (0, 1, 2):
+    row(f"rows-gather-col{_col}C", ["rows_gather_kernel"], _rows_gather, col=_col)
+row("rows-scatter", ["rows_scatter_kernel"], _rows_scatter)
+
+
+# ================================================================================================ temporal-consistency loss
+def _loss_case(N, C, h, res, seed, chunks=2):
+    flows, occs = O.synth_flows(N, res, res, seed=seed, mag=12.0)
+    ff, bf, fo, bo = O._resize_flow_occ(flows, occs, h / res)
+    assert ff.shape[-1] == h
+    g = torch.Generator(device="cuda").manual_seed(seed + 50)
+    base = torch.randn(chunks, 1, C, h, h, device="cuda", generator=g)
+    cs = (base + 0.5 * torch.randn(chunks, N, C, h, h, device="cuda", generator=g)).contiguous()   # correlated frames
+    return cs, ff.cuda().contiguous(), bf.cuda().contiguous(), (1 - fo).cuda(), (1 - bo).cuda()
+
+
+def _warp_loss(fb, launch, N, C, h, res, seed=0):
+    """fresco_warp_loss_fwd_bwd_halo (closed ring) against the oracle's formulas in fp32 on the GPU (autograd adjoint of
+    grid_sample), with the tolerance of test_temporal_loss_teacher_forced_layer_shapes."""
+    cs, ff, bf, kf, kb = _loss_case(N, C, h, res, seed=seed + h + C)
+    chunks = cs.shape[0]
+    adj = fb.ops.warp_adjoint_pair(bf, ff)
+    grad = torch.full_like(cs, float("nan"))
+    loss = torch.zeros(1, device="cuda")
+    fb.ops.warp_loss_fwd_bwd(cs, ff, bf, kf.reshape(N, h, h).contiguous(), kb.reshape(N, h, h).contiguous(), grad, loss,
+                             adjoint=adj)
+    launch("fresco_warp_loss_fwd_bwd_halo")
+    loss_ref, grad_ref = O.temporal_loss_and_grad(cs, ff.repeat(chunks, 1, 1, 1), bf.repeat(chunks, 1, 1, 1),
+                                                  kf.repeat(chunks, 1, 1, 1), kb.repeat(chunks, 1, 1, 1))
+    unwritten = (~torch.isfinite(grad)).sum().item()
+    assert unwritten == 0, f"{unwritten} gradient elements not written"
+    assert abs(loss.item() - float(loss_ref)) < 1e-4 * abs(float(loss_ref)), (loss.item(), float(loss_ref))
+    gmax = grad_ref.abs().max().item()
+    # elements whose residual is within rounding of zero may flip a sign; everything else agrees to the 16-bit adjoint
+    # weights
+    bad = ((grad - grad_ref).abs() > 1e-3 * gmax).float().mean().item()
+    assert bad < 1e-4, bad
+    cos = F.cosine_similarity(grad.flatten(), grad_ref.flatten(), dim=0).item()
+    assert cos > 0.9999, cos
+
+
+# the quad kernel: 4 NQ channel planes per CTA (channels % (4 NQ) == 0, NQ > 1 only with a grid of >= one CTA per SM)
+row("loss-quad-16x1280x32x32", ["warp_loss_quad_kernel<1,4>"], _warp_loss, N=8, C=1280, h=32, res=512)
+row("loss-quad-16x1280x12x12", ["warp_loss_quad_kernel<1,4>"], _warp_loss, N=8, C=1280, h=12, res=768)
+row("loss-quad-16x1280x24x24", ["warp_loss_quad_kernel<1,4>"], _warp_loss, N=8, C=1280, h=24, res=768)
+row("loss-quad-16x640x32x32", ["warp_loss_quad_kernel<2,2>"], _warp_loss, N=8, C=640, h=32, res=512)
+row("loss-quad-16x640x40x40", ["warp_loss_quad_kernel<2,2>"], _warp_loss, N=8, C=640, h=40, res=320)
+row("loss-quad-16x640x64x64", ["warp_loss_quad_kernel<4,1>"], _warp_loss, N=8, C=640, h=64, res=512)
+row("loss-quad-16x1280x48x48", ["warp_loss_quad_kernel<4,1>"], _warp_loss, N=8, C=1280, h=48, res=768)
+# the channel-grouped kernel: P = ceil(hw / 512) pixels x KT planes per thread; KT > 1 only with >= 296 CTAs.
+# Channel counts that are not multiples of 4 keep the quad kernel out.
+for _h, _P in ((16, 1), (32, 2), (36, 3), (40, 4)):
+    for _C, _KT in ((1190 if _h == 16 else 650, 4), (650 if _h == 16 else 450, 2), (6, 1)):
+        row(f"loss-group-P{_P}-KT{_KT}-6x{_C}x{_h}x{_h}", [f"warp_loss_group_kernel<{_P},{_KT}>"], _warp_loss, N=3, C=_C,
+            h=_h, res=8 * _h)
+for _h, _P in ((48, 5), (64, 8)):
+    for _C, _KT in ((450, 2), (6, 1)):
+        row(f"loss-group-P{_P}-KT{_KT}-6x{_C}x{_h}x{_h}", [f"warp_loss_group_kernel<{_P},{_KT}>"], _warp_loss, N=3, C=_C,
+            h=_h, res=8 * _h)
+row("loss-group-16x640x96x96", ["warp_loss_group_kernel<18,1>"], _warp_loss, N=8, C=640, h=96, res=768)
+# one CTA per plane: plane sizes no group instantiation takes (P = 7, P = 20)
+row("loss-one-cta-6x6x56x56", ["warp_loss_kernel"], _warp_loss, N=3, C=6, h=56, res=448)
+row("loss-one-cta-6x4x100x100", ["warp_loss_kernel"], _warp_loss, N=3, C=4, h=100, res=800)
+
+
+# ================================================================================================ warp chain
+def _chain_ref(sample, bwd, fwd_last, blend, chunks):
+    """The frame-chain loop of O.warp_tensor in fp64, with the per-pair blend weights given."""
+    B, C, h, w = sample.shape
+    n = B // chunks
+    z = sample.double().clone()
+    bf, ff, m = bwd.double(), fwd_last.double()[None], blend.double().reshape(n, 1, h, w)
+    for j in range(chunks):
+        base = n * j
+        for ii in range(n - 1):
+            warped = O.flow_warp(z[base + ii:base + ii + 1], bf[ii:ii + 1])
+            z[base + ii + 1] = z[base + ii + 1] * (1 - m[ii]) + warped[0] * m[ii]
+        warped = O.flow_warp(z[base:base + 1], ff)
+        z[base + n - 1] = z[base + n - 1] * (1 - m[n - 1]) + warped[0] * m[n - 1]
+    return z
+
+
+def _chain(fb, launch, chunks, N, C, h, w, dtype, seed=0):
+    """fresco_warp_fuse_chain.  Flows are multiples of 2^-10 px, so x + flow and the bilinear weights are exact in fp32
+    and the only fp32 rounding left is the blend arithmetic."""
+    g = torch.Generator(device="cuda").manual_seed(seed + C + h)
+    sample = torch.randn(chunks * N, C, h, w, device="cuda", generator=g).to(dtype)
+    bwd = (torch.randn(N, 2, h, w, device="cuda", generator=g) * 3 * 1024).round() / 1024
+    fwd_last = (torch.randn(2, h, w, device="cuda", generator=g) * 3 * 1024).round() / 1024
+    blend = torch.rand(N, h, w, device="cuda", generator=g)
+    out = torch.full_like(sample, float("nan"))
+    fb.ops.warp_fuse_chain(sample, bwd, fwd_last, blend, chunks, out=out)
+    launch("fresco_warp_fuse_chain")
+    ref = _chain_ref(sample, bwd, fwd_last, blend, chunks)
+    o = out.double()
+    unwritten = (~torch.isfinite(o)).sum().item()
+    assert unwritten == 0, f"{unwritten} outputs not written"
+    scale = ref.abs().max().item()
+    # fp32: blend rounding; fp16: one ulp of the stored value (the fp32 chain value can round either way near a tie)
+    tol = 1e-5 * scale + (2.0 ** -10 * ref.abs() if dtype == torch.float16 else 0.0)
+    bad = (o - ref).abs() > tol
+    assert not bad.any(), f"{bad.sum().item()} elements off, max error {(o - ref).abs().max().item():.3g}"
+
+
+def _chain_rejects_fp16_image_planes(fb, launch):
+    """Planes over 100 KB run the per-step kernel, which is fp32 only: fp16 is refused, not silently converted."""
+    x = torch.zeros(2 * 3, 3, 176, 176, device="cuda", dtype=torch.float16)
+    flow = torch.zeros(3, 2, 176, 176, device="cuda")
+    with pytest.raises(fb.lib.FrescoError, match="need float"):
+        fb.ops.warp_fuse_chain(x, flow, flow[0].contiguous(), torch.zeros(3, 176, 176, device="cuda"), 2)
+
+
+for _dt, _tn in ((torch.float32, "float"), (torch.float16, "half")):
+    for _h in (32, 16, 8):          # decoder features [16,1280,{8,16,32}^2]
+        row(f"chain-quad-{_tn}-16x1280x{_h}x{_h}", [f"warp_chain_quad_kernel<{_tn},1,4>"], _chain, chunks=2, N=8, C=1280,
+            h=_h, w=_h, dtype=_dt)
+    row(f"chain-quad-{_tn}-16x640x32x32", [f"warp_chain_quad_kernel<{_tn},2,2>"], _chain, chunks=2, N=8, C=640, h=32,
+        w=32, dtype=_dt)
+    row(f"chain-quad-{_tn}-16x640x64x64", [f"warp_chain_quad_kernel<{_tn},4,1>"], _chain, chunks=2, N=8, C=640, h=64,
+        w=64, dtype=_dt)
+    row(f"chain-group8-{_tn}-6x1190x16x16", [f"warp_chain_group_kernel<{_tn},8>"], _chain, chunks=2, N=3, C=1190, h=16,
+        w=16, dtype=_dt)
+    row(f"chain-group3-{_tn}-6x450x32x32", [f"warp_chain_group_kernel<{_tn},3>"], _chain, chunks=2, N=3, C=450, h=32,
+        w=32, dtype=_dt)
+    row(f"chain-group1-{_tn}-6x6x32x24", [f"warp_chain_group_kernel<{_tn},1>"], _chain, chunks=2, N=3, C=6, h=32, w=24,
+        dtype=_dt)
+row("chain-per-step-float-6x3x176x192", ["warp_blend_step_kernel"], _chain, chunks=2, N=3, C=3, h=176, w=192,
+    dtype=torch.float32)
+row("chain-per-step-half-rejected", [], _chain_rejects_fp16_image_planes)
+
+
+# ================================================================================================ GMFlow flow attention
+def _gmflow_flow_attention(fb, launch, B=16, L=4096, C=128, seed=0):
+    """GMFlow's flow propagation at 512 x 512: 64 x 64 tokens, V a flow field of tens of pixels."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    q = (torch.randn(B, L, C, device="cuda", generator=g) * 2.0).half()
+    k = torch.randn(B, L, C, device="cuda", generator=g).half()
+    vals = torch.randn(B, L, 2, device="cuda", generator=g) * 20.0
+    out = _nan((B, 2, L), torch.float32)
+    scale = 1.0 / math.sqrt(C)
+    launch("gmflow_flow_attention", fb.c.gmflow_flow_attention(P(q), P(k), P(vals), P(out), B, L, C, scale, fb.lib.stream()))
+    bound = 1e-4 * vals.abs().max().item()
+    for b in range(B):
+        s = (q[b].double() @ k[b].double().T) * scale
+        ref = (torch.softmax(s, -1) @ vals[b].double()).T
+        _check_close(out[b], ref, bound, f"flow attention batch {b}")
+
+
+row("gmflow-flow-attention-16x4096x128", ["tile_gemm_kernel<EPI_GMFLOW,0>"], _gmflow_flow_attention)
+
+
+# ================================================================================================ Gram loss
+def _gram(fb, launch, B, C, h, w, dense=False, weight=100.0, seed=0):
+    """The spatial-consistency loss at a layer shape, operand-exact: every fp64 reference is computed from the kernels'
+    own fp16 xhat / yhat / tsign, one batch at a time on the GPU."""
+    L = h * w
+    g = torch.Generator(device="cuda").manual_seed(seed + C + L)
+    base = torch.randn(B, C, 1, device="cuda", generator=g)
+    cs = (base + torch.randn(B, C, L, device="cuda", generator=g)).contiguous()
+    cs_ref = (base + torch.randn(B, C, L, device="cuda", generator=g)).contiguous()     # same statistics: D changes sign
+    st = fb.lib.stream()
+    # ---- row normalisation: xhat = fp16(x / |x|) token-major, norms fp32
+    normed = []
+    for src in (cs, cs_ref):
+        xhat, norms = _nan((B, L, C), torch.float16), _nan((B, L), torch.float32)
+        launch("fresco_gram_normalize", fb.c.fresco_gram_normalize(P(src), P(xhat), P(norms), B, C, L, st))
+        n64 = src.double().norm(dim=1)
+        _check_close(norms, n64, C * 2.0 ** -23 * n64.max().item(), "gram norms")
+        x64 = (src.double() / n64[:, None]).transpose(1, 2)
+        err = (xhat.double() - x64).abs()
+        assert torch.isfinite(xhat).all() and (err <= (2.0 ** -11 + C * 2.0 ** -23) * x64.abs() + 2.0 ** -25).all()
+        normed.append((xhat, norms))
+    (xhat, norms), (yhat, _) = normed
+    # ---- sign matrix with the recomputed target: D = X X^T - Y Y^T in one K = 2C contraction of exact fp16 products,
+    #      fp32 accumulation: |D_kernel - D| <= 2C * 2^-23 * sum|terms| <= 2C * 2^-22 (rows of unit norm)
+    tsign = _nan((B, L, L), torch.float16)
+    loss = torch.zeros(1, device="cuda")
+    launch("fresco_gram_sign_ref", fb.c.fresco_gram_sign_ref(P(xhat), P(yhat), P(tsign), P(loss), B, L, C, weight, st))
+    band = 2 * C * 2.0 ** -22
+    loss_ref, in_band = 0.0, 0
+    for b in range(B):
+        X, Y = xhat[b].double(), yhat[b].double()
+        D = X @ X.T - Y @ Y.T
+        t = tsign[b].double()
+        assert ((t == 2) | (t == 0) | (t == -2)).all(), f"batch {b}: tsign entries not in {{-2, 0, 2}} (unwritten: NaN)"
+        outside = D.abs() > band
+        bad = (t != 2 * torch.sign(D)) & outside
+        assert not bad.any(), f"batch {b}: {bad.sum().item()} signs wrong; " + _worst_tile(bad.double() * 2)
+        loss_ref += D.abs().sum().item()
+        in_band += (~outside).sum().item()
+        del D, t, bad, outside
+    assert in_band < 0.05 * B * L * L, f"{in_band} of {B * L * L} entries inside the accumulation band"
+    loss_ref *= weight / (B * L * L)
+    assert abs(loss.item() - loss_ref) < 1e-4 * loss_ref, (loss.item(), loss_ref)
+    # ---- ghat = alpha T X (tensor-core product of the backward), from the kernel's own T
+    alpha = weight / (B * L * L)
+    ghat = _nan((B, L, C), torch.float32)
+    launch("fresco_gram_tx", fb.c.fresco_gram_tx(P(tsign), P(xhat), P(ghat), B, L, C, alpha, st))
+    # ---- grad += projection of ghat through the normalisation Jacobian, under both products fresco_gram_grad can use
+    grad0 = torch.zeros(B, C, L, device="cuda")
+    nbytes = int(fb.c.fresco_gram_grad_workspace_bytes(B, L, C))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
+    grads = {}
+    for v in (2, 1):
+        fb.lib.set_option("FRESCO_GRAM_V", v)
+        gr = grad0.clone()
+        launch(f"fresco_gram_grad (FRESCO_GRAM_V={v})",
+               fb.c.fresco_gram_grad(P(tsign), P(xhat), P(norms), P(gr), B, L, C, weight, P(ws), nbytes, st))
+        grads[v] = gr
+    fb.lib.set_option("FRESCO_GRAM_V", -1)
+    for b in range(B):
+        T, X = tsign[b].double(), xhat[b].double()
+        g64 = alpha * (T @ X)
+        # fp32 accumulation over L terms: sqrt(L) 2^-20 of sum|terms| (16x the error of truncating accumulators), plus
+        # the rounding of the alpha product
+        e = 2.0 ** -20 * math.sqrt(L) * alpha * (T.abs() @ X.abs()) + 2.0 ** -22 * g64.abs()
+        del T
+        ratio = (ghat[b].double() - g64).abs() / e
+        assert not (ratio > 1).any() and torch.isfinite(ghat[b]).all(), f"gram_tx batch {b}: " + _worst_tile(ratio)
+        dot = (g64 * X).sum(1, keepdim=True)
+        nrm = norms[b].double()[:, None]
+        proj = (g64 - dot * X) / nrm
+        dot_err = (e * X.abs()).sum(1, keepdim=True) + C * 2.0 ** -23 * (g64 * X).abs().sum(1, keepdim=True)
+        tol = (e + X.abs() * dot_err + 2.0 ** -22 * (g64.abs() + (dot * X).abs())) / nrm
+        want = grad0[b].double().T + proj                                            # [L, C]
+        tol = tol + 2.0 ** -23 * want.abs()
+        for v, gr in grads.items():
+            ratio = (gr[b].double().T - want).abs() / tol
+            assert not (ratio > 1).any() and torch.isfinite(gr[b]).all(), \
+                f"gram_grad (FRESCO_GRAM_V={v}) batch {b}: " + _worst_tile(ratio)
+    if dense:
+        # the dense-target entry point (a caller holding the reference's fp32 correlation matrix): T = sign(G - A) +
+        # sign(G - A^T), loss over |G - A|; G from fp32 accumulation of C exact products, |G_kernel - G| <= C 2^-23
+        A = torch.empty(B, L, L, device="cuda")
+        for b in range(B):
+            A[b] = (xhat[b].double() @ xhat[b].double().T + 0.05 * torch.randn(L, L, device="cuda", generator=g,
+                                                                               dtype=torch.float64)).float()
+        tsign2 = _nan((B, L, L), torch.float16)
+        loss2 = torch.zeros(1, device="cuda")
+        launch("fresco_gram_sign", fb.c.fresco_gram_sign(P(xhat), P(A), P(tsign2), P(loss2), B, L, C, weight, st))
+        band2, ref2 = C * 2.0 ** -22, 0.0
+        for b in range(B):
+            G = xhat[b].double() @ xhat[b].double().T
+            d1, d2 = G - A[b].double(), G - A[b].double().T
+            t = tsign2[b].double()
+            assert torch.isfinite(t).all(), f"dense target batch {b}: tsign not written"
+            bad = (t != torch.sign(d1) + torch.sign(d2)) & (d1.abs() > band2) & (d2.abs() > band2)
+            assert not bad.any(), f"dense target batch {b}: " + _worst_tile(bad.double() * 2)
+            ref2 += d1.abs().sum().item()
+        ref2 *= weight / (B * L * L)
+        assert abs(loss2.item() - ref2) < 1e-4 * ref2, (loss2.item(), ref2)
+
+
+_GRAM_KERNELS = ["gram_normalize_kernel", "gram_normalize_kernel", "gram2_kernel<G2_SIGN>", "gram2_kernel<G2_GRAD>",
+                 "gram_project_kernel", "gram_project_kernel"]
+row("gram-16x640x64x64", _GRAM_KERNELS, _gram, opts={"FRESCO_GRAM_V": -1}, B=16, C=640, h=64, w=64)
+row("gram-16x1280x32x32", _GRAM_KERNELS + ["tile_gemm_kernel<EPI_GRAM_SIGN,0>"], _gram, opts={"FRESCO_GRAM_V": -1}, B=16, C=1280, h=32, w=32,
+    dense=True)
+row("gram-16x640x96x96", _GRAM_KERNELS, _gram, opts={"FRESCO_GRAM_V": -1}, B=16, C=640, h=96, w=96)
+row("gram-4x16x24x24", _GRAM_KERNELS + ["tile_gemm_kernel<EPI_GRAM_SIGN,0>"], _gram, opts={"FRESCO_GRAM_V": -1}, B=4, C=16, h=24, w=24, dense=True)
+
+
+# ================================================================================================ what no row reaches
+_QUAD_NEVER = ("quad_config starts P at 4 / NQ and only doubles it (P * NQ >= 4), so it never returns this (P, NQ)")
+UNREACHABLE = {}
+for _pq in ("1,2", "2,1", "1,1"):
+    UNREACHABLE[f"warp_loss_quad_kernel<{_pq}>"] = _QUAD_NEVER
+    for _tn in ("float", "half"):
+        UNREACHABLE[f"warp_chain_quad_kernel<{_tn},{_pq}>"] = _QUAD_NEVER
+NOT_LAST = {
+    "tile_gemm_kernel<EPI_STORE,1>": "fresco_gram_grad under FRESCO_GRAM_V=1 launches it before gram_project_kernel; the "
+                                     "gram rows check the gradient it feeds elementwise under that option",
+}
+COVERED_ELSEWHERE = {
+    "kv_compact_kernel": "test_gpu_kernels.py::test_kv_compact_bit_exact",
+    "flow_warp_kernel": "test_gpu_kernels.py::test_flow_warp_and_consistency",
+    "warp_taps_kernel": "builds the adjoint of every temporal-loss row here, checked through their gradients",
+    "adam_kernel": "test_gpu_kernels.py::test_adam_matches_torch",
+    "adain_kernel<half>": "test_gpu_kernels.py::test_adain_eps_quirk",
+    "adain_kernel<float>": "test_gpu_kernels.py::test_adain_eps_quirk",
+    "cfg_pred_x0_kernel<half>": "test_gpu_parity_r2.py::test_ddpm_step_kernels_and_dilate_golden",
+    "cfg_pred_x0_kernel<float>": "test_gpu_parity_r2.py::test_ddpm_step_kernels_and_dilate_golden",
+    "ddpm_prev_kernel<half>": "test_gpu_parity_r2.py::test_ddpm_step_kernels_and_dilate_golden",
+    "ddpm_prev_kernel<float>": "test_gpu_parity_r2.py::test_ddpm_step_kernels_and_dilate_golden",
+    "dilate_kernel": "test_gpu_parity_r2.py::test_ddpm_step_kernels_and_dilate_golden",
+    "to_token_major_f16_kernel": "test_gpu_kernels.py::test_gmflow_global_correlation (first launches of the call)",
+    "mapping_single_kernel": "test_gpu_kernels.py::test_mapping_bit_exact_golden",
+}
+
+
+def _table_names():
+    return {k for r in ROWS for k in r.kernels}
+
+
+def _source_names():
+    """Launch names the launchers can produce, from the instantiation lists in the sources."""
+    src = {f: open(os.path.join(CSRC, f)).read() for f in os.listdir(CSRC) if f.endswith(".cu")}
+    hbm, attn = src["hbm_kernels.cu"], src["attn_wgmma.cu"]
+    names = set()
+    for p, q in re.findall(r"\bLQ\((\d+), (\d+)\)", hbm):
+        names.add(f"warp_loss_quad_kernel<{p},{q}>")
+    for p, k in re.findall(r"\bLOSS_CASE\((\d+), (\d+)\)", hbm):
+        names.add(f"warp_loss_group_kernel<{p},{k}>")
+    for tn in ("float", "half"):
+        for p, q in re.findall(r"\bCQ\((\d+), (\d+)\)", hbm):
+            names.add(f"warp_chain_quad_kernel<{tn},{p},{q}>")
+        for k in re.findall(r"launch_chain_group<T, (\d+)>", hbm):
+            names.add(f"warp_chain_group_kernel<{tn},{k}>")
+    nmax = re.findall(r"launch_temporal_rows<DD, (\d+)>", hbm)
+    for d in re.findall(r"\bROWS\((\d+)\);", hbm):
+        names.update(f"temporal_attn_rows_kernel<{d},{n}>" for n in nmax)
+    for d in map(int, re.findall(r"\bATTN_CASE\((\d+)\);", attn)):
+        for wide in ((0, 1, 2) if d <= 64 else (0, 1)):
+            for poly in (0, 4, 8):
+                for rowsum in ((0, 1) if wide == 0 else (0,)):
+                    names.add(attn_name(d, wide, poly, rowsum))
+    for epi, bmn in re.findall(r"launch_gemm<(EPI_\w+), (true|false)>", src["gemm_wgmma.cu"]):
+        names.add(f"tile_gemm_kernel<{epi},{int(bmn == 'true')}>")
+    names.update(re.findall(r"\"(gram2_kernel<G2_\w+>)\"", src["gram_wgmma.cu"]))
+    # plain launch names: check_launch("name") / check_launch(c ? "name<half>" : "name<float>")
+    for text in src.values():
+        for call in re.findall(r"check_launch\(([^;]*)\);", text):
+            names.update(re.findall(r"\"(\w+_kernel(?:<\w+>)?)\"", call))
+    return names
+
+
+def test_launch_name_universe():
+    """Every launch name the sources can produce is a table row, unreachable, not the last launch of its call, or
+    checked by a named test elsewhere -- exactly one of those; a new kernel or instantiation fails here until it is
+    placed.  (Needs no GPU.)"""
+    table = _table_names()
+    buckets = [table, set(UNREACHABLE), set(NOT_LAST), set(COVERED_ELSEWHERE)]
+    for i in range(len(buckets)):
+        for j in range(i + 1, len(buckets)):
+            assert not buckets[i] & buckets[j], buckets[i] & buckets[j]
+    known = set().union(*buckets)
+    universe = _source_names()
+    assert len(universe) > 80, len(universe)
+    assert universe == known, {"not placed": sorted(universe - known), "not launchable": sorted(known - universe)}
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("r", ROWS, ids=lambda r: r.id)
+def test_kernel_variant(fb, r):
+    for name, v in r.opts.items():
+        fb.lib.set_option(name, v)
+    try:
+        launch = Launches(fb, r)
+        r.run(fb, launch)
+        assert launch.i == len(r.kernels), f"launched {launch.i} of the {len(r.kernels)} kernels the table expects"
+    finally:
+        for name in r.opts:
+            fb.lib.set_option(name, -1)
+        torch.cuda.empty_cache()
+    RAN.add(r.id)
+
+
+@pytest.mark.gpu
+def test_every_reachable_name_was_launched(fb):
+    """The names the rows saw are exactly the table's reachable set (runs after the rows, with all of them)."""
+    if len(RAN) != len(ROWS):
+        pytest.skip("only meaningful after every row has run and passed")
+    assert SEEN == _table_names(), {"expected, not seen": sorted(_table_names() - SEEN), "seen": sorted(SEEN - _table_names())}

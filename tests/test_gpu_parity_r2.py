@@ -331,14 +331,15 @@ def test_temporal_loss_adjoint_overflow_path(fb):
 
 
 @pytest.mark.parametrize("N,C,h,world", [(8, 640, 64, 2), (8, 1280, 16, 4), (8, 1280, 8, 8), (6, 6, 24, 3), (8, 6, 32, 2),
-                                         (4, 4, 100, 2)])
+                                         (4, 4, 100, 2), (8, 640, 96, 2)])
 def test_temporal_loss_open_chain_equals_ring(fb, N, C, h, world):
     """Exchange 3 of the frame partition (SURVEY 8e): every "rank" evaluates its own pairs with the following rank's first
     frame as halo (fresco_warp_loss_fwd_bwd_halo) and hands the halo gradient on; the assembled gradient must be
     BIT-identical to the closed ring over all N frames, ELL overflow lists included (they are summed in list order, no
-    atomics) -- quad kernel, channel-grouped kernel (C = 6 / 24) and the one-plane-per-CTA kernel (100 x 100 planes;
-    that one associates the overflow terms differently, so it is bit-identical only when no ELL row overflows)."""
-    flows, occs, cs = _layer_case(N, C, h, seed=7 * h + world, res=800 if h == 100 else 512)
+    atomics) -- quad kernel, channel-grouped kernel (C = 6 / 24; config 5's 96 x 96 planes: P = 18) and the
+    one-plane-per-CTA kernel (100 x 100 planes; that one associates the overflow terms differently, so it is
+    bit-identical only when no ELL row overflows)."""
+    flows, occs, cs = _layer_case(N, C, h, seed=7 * h + world, res={100: 800, 96: 768}.get(h, 512))
     ff, bf, fo, bo = O._resize_flow_occ(flows, occs, h / flows[0].shape[2])
     dev = "cuda"
     cs = cs.to(dev)
