@@ -8,17 +8,30 @@
 // 128B-swizzled K-major layout; columns >= head_dim and rows >= tokens are hardware zero-filled (no padding passes for
 // head_dim 40 / 80 or ragged lengths).
 //
-//   last warp     TMA producer: Q once, K/V tiles of KN keys through an mbarrier ring of as many stages (<= 4) as fit
-//   NWG x 4 warps consumer warpgroups, 64 query rows each.  Per key tile: S = Q K^T by wgmma (A and B from shared
-//                 memory, fp32 accumulators in registers), online softmax in registers (a query row lives in the four
-//                 lanes of a quad), P converted to fp16 A fragments in registers, O += P V by wgmma with A from registers
-//                 and V read MN-major from the same swizzled tile.  The warpgroups drift apart, so the tensor core
-//                 works for one while the others are in their exponentials.
+//   last warpgroup  TMA producer: Q once, K/V tiles of KN keys through an mbarrier ring of as many stages (<= 4) as
+//                   fit.  One elected thread issues; the warpgroup drops to 24 registers (setmaxnreg) so the
+//                   consumers can have 240 (NWG = 2) or 160 (NWG = 3).
+//   NWG consumer warpgroups, 64 query rows each.  Per key tile: S = Q K^T by wgmma (A and B from shared memory, fp32
+//                   accumulators in registers), online softmax in registers (a query row lives in the four lanes of a
+//                   quad), P converted to fp16 A fragments in registers, O += P V by wgmma with A from registers and V
+//                   read MN-major from the same swizzled tile.
+//
+// Two schedules keep the tensor core busy while the SFU computes exponentials:
+//   software pipeline  turn t issues S_t = Q K_t^T and O += P_{t-1} V_{t-1} together, waits for S_t only
+//                      (wgmma_wait<1>) and computes its softmax while the P V runs; O is rescaled after the P V has
+//                      retired, and ring stage t-1 is released then.  A prologue turn issues S_0 alone, an epilogue turn
+//                      the last P V alone.
+//   ping-pong          a token passes round the consumer warpgroups on named barriers 1..NWG: warpgroup w issues its
+//                      GEMMs of a turn only after warpgroup w-1 has issued its own, so while one warpgroup is in its
+//                      exponentials the next one's GEMMs run.  Every warpgroup takes all n_tiles + 1 turns, also when
+//                      its rows are past q_len, so the ring never stalls.
+//
+// Softmax: the row max is taken on the raw scores (softmax_scale > 0) and the exponent is one FFMA,
+// s * scale_log2 - m * scale_log2.  Tiles that hold the ragged tail or the diagonal take a separate masking pass.
 //
 // Variants (fresco_set_option / environment, read once; every one is parity-tested at every head_dim):
 //   FRESCO_ATTN_WIDE    0: 64-key tiles, two consumer warpgroups; 1 (default): 128-key tiles, two warpgroups;
-//                       2: 128-key tiles, three warpgroups (192 query rows per CTA; head_dim <= 64, else as 1:
-//                       at 80 the 416-thread CTA runs out of registers)
+//                       2: 128-key tiles, three warpgroups (192 query rows per CTA; head_dim <= 64, else as 1)
 //   FRESCO_ATTN_POLY    0 (default) | 4 | 8: every n-th pair of exponentials by a polynomial on the FMA pipe
 //                       instead of MUFU.EX2
 //   FRESCO_ATTN_ROWSUM  64-key tiles only: row sums from the tensor core (one m64n8 wgmma of P against a tile of
@@ -31,14 +44,16 @@ namespace fresco {
 template <int D, int KN, int NWG, bool ROWSUM>
 struct AttnCfg {
   static constexpr int TILE_M = 64 * NWG;             // query rows per CTA
-  static constexpr int THREADS = 128 * NWG + 32;
+  static constexpr int THREADS = 128 * (NWG + 1);
+  static constexpr int PRODUCER_REGS = 24;            // 128 * 24 + 128 * NWG * CONSUMER_REGS <= 65536
+  static constexpr int CONSUMER_REGS = NWG == 2 ? 240 : 160;
+  static constexpr int LAUNCH_REGS = 65536 / THREADS / 8 * 8;   // what ptxas gives every thread at launch
   static constexpr int Q_ATOM = TILE_M * 128;         // [TILE_M rows x 64 fp16]
   static constexpr int KV_ATOM = KN * 128;            // [KN rows x 64 fp16]
   static constexpr int NATOM = (D + 63) / 64;
-  static constexpr int KSTEPS = (D + 15) / 16;
-  static constexpr int DPAD = KSTEPS * 16;
-  static constexpr int N0 = DPAD < 64 ? DPAD : 64;   // P V columns from atom 0
-  static constexpr int N1 = DPAD - N0;               // P V columns from atom 1
+  static constexpr int KSTEPS = (D + 15) / 16;        // Q K^T: columns past D are zero-filled by TMA
+  static constexpr int N0 = D < 64 ? D : 64;          // P V columns from atom 0 (every D is a multiple of 8)
+  static constexpr int N1 = D - N0;                   // P V columns from atom 1
   static constexpr int Q_BYTES = NATOM * Q_ATOM;
   static constexpr int STAGE_BYTES = 2 * NATOM * KV_ATOM;
   static constexpr int ONES_BYTES = ROWSUM ? 2048 : 0;  // [16 keys x 64] fp16 ones: B operand of the row-sum wgmma
@@ -53,7 +68,7 @@ struct AttnParams {
   __half* out;
   int q_len, kv_len, heads, q_per_kv;
   float scale_log2;        // softmax_scale * log2(e)
-  float diag_bias_log2;    // bias added where kv index == query index, * log2(e)
+  float diag_bias;         // bias added to the raw score where kv index == query index: diag_bias / softmax_scale
 };
 
 // exp2 on the FMA pipe (POLY variants): Cody-Waite split x = n + f, f in [-0.5, 0.5], degree-3 minimax polynomial for
@@ -116,9 +131,10 @@ fresco_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
   }
   __syncthreads();
 
-  if (warp == 4 * NWG) {
-    // ------------------------------------------------------------ TMA producer
-    if (FRESCO_ISSUER_THREAD(lane)) {
+  if (warp >= 4 * NWG) {
+    // ------------------------------------------------------------ TMA producer warpgroup
+    setmaxnreg_dec<Cfg::PRODUCER_REGS>();
+    if (warp == 4 * NWG && FRESCO_ISSUER_THREAD(lane)) {
       tma_prefetch_desc(&tm_q);
       tma_prefetch_desc(&tm_k);
       tma_prefetch_desc(&tm_v);
@@ -140,29 +156,26 @@ fresco_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
   }
 
   // -------------------------------------------------------------- consumer warpgroups
+  setmaxnreg_inc<Cfg::CONSUMER_REGS>();
   const int wg = warp >> 2;
   const int row0 = q0 + wg * 64 + acc_row(0);      // this thread's two query rows: row0, row0 + 8
-  const float scale_log2 = p.scale_log2, bias_log2 = p.diag_bias_log2;
-  const bool use_bias = bias_log2 != 0.f;
+  const float scale_log2 = p.scale_log2, bias = p.diag_bias;
+  const bool use_bias = bias != 0.f;
   float o0[Cfg::N0 / 2], o1[Cfg::N1 > 0 ? Cfg::N1 / 2 : 1];
 #pragma unroll
   for (int i = 0; i < Cfg::N0 / 2; ++i) o0[i] = 0.f;
 #pragma unroll
   for (int i = 0; i < (Cfg::N1 > 0 ? Cfg::N1 / 2 : 1); ++i) o1[i] = 0.f;
-  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // m_run: raw scores
   float l_acc[4] = {0.f, 0.f, 0.f, 0.f};           // ROWSUM: every column of the m64n8 accumulator is the row sum
   const uint32_t q_addr = smem_u32(s_q) + wg * 64 * 128;
+  float s[kTileN / 2];                             // S_t, then P_t in fp32
+  uint32_t pa[kTileN / 16][4];                     // P_t as fp16 A fragments, read by the P V wgmma of the next turn
+  float alpha[2];                                  // rescale of O and l from the previous running max to this tile's
 
-  mbar_wait_mma(bar_q, 0);
-  for (int t = 0; t < n_tiles; ++t) {
-    const int st = t % ST;
-    mbar_wait_mma(bar_full + st, (t / ST) & 1);
-    const uint32_t k_addr = smem_u32(s_kv + st * Cfg::STAGE_BYTES);
-    const uint32_t v_addr = k_addr + Cfg::NATOM * kKVAtomBytes;
-
-    // ---- S = Q K^T  (64 x 128 per warpgroup)
-    float s[kTileN / 2];
-    wgmma_fence();
+  // S = Q K^T of tile t into s (not committed)
+  auto issue_qk = [&](int t) {
+    const uint32_t k_addr = smem_u32(s_kv + (t % ST) * Cfg::STAGE_BYTES);
 #pragma unroll
     for (int ks = 0; ks < Cfg::KSTEPS; ++ks) {
       const uint32_t qoff = (ks >> 2) * kQAtomBytes + (ks & 3) * 32;
@@ -170,63 +183,10 @@ fresco_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
       wgmma_ss<kTileN>(s, make_smem_desc_sw128(q_addr + qoff, 16, 1024), make_smem_desc_sw128(k_addr + koff, 16, 1024),
                        ks > 0 ? 1u : 0u);
     }
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(s);
-
-    // ---- scale, mask the ragged tail, diagonal bias (all in the log2 domain)
-    const int col0 = t * kTileN;
-    const bool special = (col0 + kTileN > p.kv_len) || (use_bias && q0 < col0 + kTileN && q0 + kTileM > col0);
-#pragma unroll
-    for (int i = 0; i < kTileN / 2; ++i) s[i] *= scale_log2;
-    if (special) {
-#pragma unroll
-      for (int i = 0; i < kTileN / 2; ++i) {
-        const int col = col0 + acc_col(i);
-        const int row = row0 + 8 * ((i >> 1) & 1);
-        if (use_bias && col == row) s[i] += bias_log2;
-        if (col >= p.kv_len) s[i] = -INFINITY;
-      }
-    }
-    // ---- online softmax: row max over the quad, rescale O and l, p = exp2(s - m)
-    float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int i = 0; i < kTileN / 2; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
-    float alpha[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      const float m_new = fmaxf(m_run[r], quad_max(mx[r]));
-      alpha[r] = fast_exp2(m_run[r] - m_new);
-      m_run[r] = m_new;
-      l_run[r] *= alpha[r];
-    }
-#pragma unroll
-    for (int i = 0; i < kTileN / 2; ++i) {
-      const float x = s[i] - m_run[(i >> 1) & 1];
-      s[i] = (POLY > 0 && ((i >> 1) % (POLY > 0 ? POLY : 1)) == POLY - 1) ? exp2_poly(x) : fast_exp2(x);
-      if (!ROWSUM) l_run[(i >> 1) & 1] += s[i];
-    }
-    if (ROWSUM) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) l_acc[i] *= alpha[(i >> 1) & 1];
-    }
-#pragma unroll
-    for (int i = 0; i < Cfg::N0 / 2; ++i) o0[i] *= alpha[(i >> 1) & 1];
-    if (Cfg::N1 > 0) {
-#pragma unroll
-      for (int i = 0; i < Cfg::N1 / 2; ++i) o1[i] *= alpha[(i >> 1) & 1];
-    }
-
-    // ---- O += P V: P (fp16) as register A fragments, 16 keys per step
-    uint32_t pa[kTileN / 16][4];
-#pragma unroll
-    for (int k2 = 0; k2 < kTileN / 16; ++k2)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) pa[k2][j] = pack_half2(s[8 * k2 + 2 * j], s[8 * k2 + 2 * j + 1]);
-    reg_fence(o0);
-    reg_fence(o1);
-    reg_fence(l_acc);
-    wgmma_fence();
+  };
+  // O += P V of tile t from pa, 16 keys per step (not committed)
+  auto issue_pv = [&](int t) {
+    const uint32_t v_addr = smem_u32(s_kv + (t % ST) * Cfg::STAGE_BYTES) + Cfg::NATOM * kKVAtomBytes;
 #pragma unroll
     for (int k2 = 0; k2 < kTileN / 16; ++k2) {
       wgmma_rs<Cfg::N0>(o0, pa[k2], make_smem_desc_sw128(v_addr + k2 * 2048, kKVAtomBytes, 1024), 1u);
@@ -235,19 +195,115 @@ fresco_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
       if constexpr (ROWSUM)   // l += P_t * ones  (every element of the tile is 1.0, so its layout is moot)
         wgmma_rs<8>(l_acc, pa[k2], make_smem_desc_sw128(smem_u32(s_ones), 2048, 1024), 1u);
     }
-    wgmma_commit();
-    wgmma_wait<0>();
+  };
+  // online softmax of tile t in s: mask, running max, alpha, p = exp2(s * scale_log2 - m * scale_log2), row sums
+  auto softmax = [&](int t) {
+    const int col0 = t * kTileN;
+    const bool special = (col0 + kTileN > p.kv_len) || (use_bias && q0 < col0 + kTileN && q0 + kTileM > col0);
+    if (special) {
+#pragma unroll
+      for (int i = 0; i < kTileN / 2; ++i) {
+        const int col = col0 + acc_col(i);
+        const int row = row0 + 8 * ((i >> 1) & 1);
+        if (use_bias && col == row) s[i] += bias;
+        if (col >= p.kv_len) s[i] = -INFINITY;
+      }
+    }
+    float mx[2] = {m_run[0], m_run[1]};
+#pragma unroll
+    for (int i = 0; i < kTileN / 2; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
+    float neg_ms[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {   // column col0 is a key of every row, so m_new is finite
+      const float m_new = quad_max(mx[r]);
+      alpha[r] = fast_exp2((m_run[r] - m_new) * scale_log2);
+      m_run[r] = m_new;
+      neg_ms[r] = -m_new * scale_log2;
+      l_run[r] *= alpha[r];
+    }
+#pragma unroll
+    for (int i = 0; i < kTileN / 2; ++i) {
+      const float x = fmaf(s[i], scale_log2, neg_ms[(i >> 1) & 1]);
+      s[i] = (POLY > 0 && ((i >> 1) % (POLY > 0 ? POLY : 1)) == POLY - 1) ? exp2_poly(x) : fast_exp2(x);
+      if (!ROWSUM) l_run[(i >> 1) & 1] += s[i];
+    }
+  };
+  // after the P V of the previous tile has retired: rescale O (and l), P_t -> fp16 fragments
+  auto rescale_and_pack = [&]() {
+#pragma unroll
+    for (int i = 0; i < Cfg::N0 / 2; ++i) o0[i] *= alpha[(i >> 1) & 1];
+    if constexpr (Cfg::N1 > 0) {
+#pragma unroll
+      for (int i = 0; i < Cfg::N1 / 2; ++i) o1[i] *= alpha[(i >> 1) & 1];
+    }
+    if constexpr (ROWSUM) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) l_acc[i] *= alpha[(i >> 1) & 1];
+    }
+#pragma unroll
+    for (int k2 = 0; k2 < kTileN / 16; ++k2)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) pa[k2][j] = pack_half2(s[8 * k2 + 2 * j], s[8 * k2 + 2 * j + 1]);
+  };
+  auto fence_acc = [&]() {
     reg_fence(o0);
     reg_fence(o1);
     reg_fence(l_acc);
+  };
+  auto release = [&](int t) {      // this warp's reads of K_t and V_t are complete
     __syncwarp();
-    if (lane == 0) mbar_arrive(bar_empty + st);   // this warp's reads of K_t and V_t are complete
+    if (lane == 0) mbar_arrive(bar_empty + t % ST);
+  };
+  // ping-pong turns: barrier 1 + w is warpgroup w's; it completes when w and w-1 (128 threads each) have arrived
+  const int bar_mine = 1 + wg, bar_next = 1 + (wg + 1) % NWG;
+  if (wg == NWG - 1) named_bar_arrive(1, 256);     // warpgroup 0 takes the first turn
+
+  mbar_wait_mma_raised<Cfg::LAUNCH_REGS>(bar_q, 0);
+  // ---- prologue turn: S_0
+  mbar_wait_mma_raised<Cfg::LAUNCH_REGS>(bar_full, 0);
+  named_bar_sync(bar_mine, 256);
+  wgmma_fence();
+  issue_qk(0);
+  wgmma_commit();
+  named_bar_arrive(bar_next, 256);
+  wgmma_wait<0>();
+  reg_fence(s);
+  softmax(0);
+  rescale_and_pack();
+  // ---- turn t: S_t and O += P_{t-1} V_{t-1} in flight together; softmax of S_t overlaps the P V
+  for (int t = 1; t < n_tiles; ++t) {
+    mbar_wait_mma_raised<Cfg::LAUNCH_REGS>(bar_full + t % ST, (t / ST) & 1);
+    named_bar_sync(bar_mine, 256);
+    fence_acc();
+    wgmma_fence();
+    issue_qk(t);
+    wgmma_commit();
+    issue_pv(t - 1);
+    wgmma_commit();
+    named_bar_arrive(bar_next, 256);
+    wgmma_wait<1>();
+    reg_fence(s);
+    softmax(t);
+    wgmma_wait<0>();
+    fence_acc();
+    release(t - 1);
+    rescale_and_pack();
   }
+  // ---- epilogue turn: the last P V.  The ring ends here: warpgroup NWG-1 passes no token to warpgroup 0.
+  named_bar_sync(bar_mine, 256);
+  fence_acc();
+  wgmma_fence();
+  issue_pv(n_tiles - 1);
+  wgmma_commit();
+  if (wg != NWG - 1) named_bar_arrive(bar_next, 256);
+  wgmma_wait<0>();
+  fence_acc();
+  release(n_tiles - 1);
 
   // ---- epilogue: O / l -> fp16 head slice of the two rows
   float inv[2];
 #pragma unroll
-  for (int r = 0; r < 2; ++r) inv[r] = 1.f / (ROWSUM ? l_acc[2 * r] : quad_sum(l_run[r]));
+  for (int r = 0; r < 2; ++r) inv[r] = __fdividef(1.f, ROWSUM ? l_acc[2 * r] : quad_sum(l_run[r]));   // l >= 1
   const size_t row_elems = static_cast<size_t>(p.heads) * D;
   __half* dst = p.out + static_cast<size_t>(b) * p.q_len * row_elems + static_cast<size_t>(head) * D;
 #pragma unroll
@@ -377,7 +433,7 @@ static int launch_attn(const void* q, const void* k, const void* v, void* out, i
   p.heads = heads;
   p.q_per_kv = q_per_kv;
   p.scale_log2 = softmax_scale * 1.4426950408889634f;
-  p.diag_bias_log2 = diag_bias * 1.4426950408889634f;
+  p.diag_bias = diag_bias / softmax_scale;
   const AttnVariant a = attn_variant(D);
 #define ATTN_ARGS q, k, v, out, batch_q, q_len, kv_len, heads, q_per_kv, kv_row_stride, kv_batch_stride, p, stream
   if (a.wide == 0)

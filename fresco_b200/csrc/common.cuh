@@ -1,5 +1,6 @@
 // Thin inline-PTX wrappers for the sm_90a features the kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / commit / wait; the MMAs themselves are in wgmma.cuh).
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / commit / wait; the MMAs themselves are in wgmma.cuh),
+// setmaxnreg and named barriers.
 // The bit layout of the matrix descriptor follows the PTX ISA "wgmma matrix descriptor" table.
 #pragma once
 #include <cuda.h>
@@ -144,6 +145,33 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// ---------------------------------------------------------------- warpgroup scheduling
+// setmaxnreg: every warp of a warpgroup executes the same one; the kernel needs __launch_bounds__ so ptxas knows the
+// register count it starts from.  The values are multiples of 8 in [24, 256].
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+// named barriers (id 0 is __syncthreads'): a barrier completes when `threads` threads have arrived; bar.sync arrives
+// and waits, bar.arrive only arrives.
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+// mbar_wait_mma for a warpgroup that raised its register budget with setmaxnreg.inc: ptxas holds every region from
+// which a trap is reachable to the launch-time register count, so the watchdog first drops back to LAUNCH_REGS.
+template <int LAUNCH_REGS>
+__device__ __forceinline__ void mbar_wait_mma_raised(uint64_t* bar, uint32_t parity) {
+  uint32_t polls = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++polls > FRESCO_WATCHDOG_POLLS) {
+      setmaxnreg_dec<LAUNCH_REGS>();
+      __trap();
+    }
+  }
+}
 // keeps the compiler from moving reads or writes of accumulator registers across an asynchronous wgmma
 template <int N>
 __device__ __forceinline__ void reg_fence(float (&r)[N]) {
