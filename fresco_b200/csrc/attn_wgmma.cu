@@ -382,13 +382,8 @@ static int launch_variant(const void* q, const void* k, const void* v, void* out
   if (make_head_tile_map(&tq, q, D, heads, q_len, batch_q, Cfg::TILE_M, C, C * q_len)) return FRESCO_ERR_TENSORMAP;
   if (make_head_tile_map(&tk, k, D, heads, kv_len, batch_kv, KN, kv_row_stride, kv_batch_stride)) return FRESCO_ERR_TENSORMAP;
   if (make_head_tile_map(&tv, v, D, heads, kv_len, batch_kv, KN, kv_row_stride, kv_batch_stride)) return FRESCO_ERR_TENSORMAP;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(fresco_attn_kernel<D, KN, NWG, POLY, ROWSUM>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(attn)");
-    attr_set = true;
-  }
+  if (int rc = allow_dynamic_smem((const void*)fresco_attn_kernel<D, KN, NWG, POLY, ROWSUM>, Cfg::SMEM_BYTES, "attn"))
+    return rc;
   dim3 grid((q_len + Cfg::TILE_M - 1) / Cfg::TILE_M, heads, batch_q);
   fresco_attn_kernel<D, KN, NWG, POLY, ROWSUM><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(tq, tk, tv, p);
   return check_launchf(ATTN_NAME_FMT, D, KN, NWG, POLY, ROWSUM ? ",rowsum" : "");

@@ -20,7 +20,17 @@ int check_launchf(const char* fmt, ...) __attribute__((format(printf, 1, 2)));
 int encode_tiled_map(CUtensorMap* map, CUtensorMapDataType dtype, int rank, void* base, const cuuint64_t* dims,
                      const cuuint64_t* strides_bytes, const cuuint32_t* box, const cuuint32_t* elem_strides,
                      CUtensorMapSwizzle swizzle);
+// fp16 GEMM operands, 128-byte swizzle.  K-major [batch, rows, K] -> {K, rows, batch}, box {64, box_rows, 1};
+// MN-major [batch, K rows, N cols] -> {N, K, batch}, box {64, 64, 1}
+int make_kmajor_map(CUtensorMap* map, const void* base, int rows, int K, int batch, int box_rows);
+int make_mnmajor_map(CUtensorMap* map, const void* base, int K, int N, int batch);
 
+// Lets `kernel` launch with up to `bytes` of dynamic shared memory on the current device.  The attribute is set once
+// per (kernel, device), raised only when a larger amount is asked for, and never needed at or below the 48 KB
+// default; thread-safe.  Failure is reported through set_cuda_error, naming `what`.
+int allow_dynamic_smem(const void* kernel, size_t bytes, const char* what);
+
+// multiprocessor count of the current device, looked up once per device
 int sm_count();
 
 // Tuning options: each has the name of an environment variable, which is read ONCE (first use); fresco_set_option()

@@ -211,33 +211,9 @@ tile_gemm_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
   }
 }
 
-// K-major operand [batch, rows, K] fp16 -> {K, rows, batch}, box {64, 128, 1}
-static int make_kmajor_map(CUtensorMap* map, const void* base, int rows, int K, int batch) {
-  const cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)rows, (cuuint64_t)batch};
-  const cuuint64_t strides[2] = {(cuuint64_t)K * 2, (cuuint64_t)rows * K * 2};
-  const cuuint32_t box[3] = {64, 128, 1};
-  const cuuint32_t es[3] = {1, 1, 1};
-  return encode_tiled_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, es,
-                          CU_TENSOR_MAP_SWIZZLE_128B);
-}
-// MN-major B operand [batch, K rows, N cols] fp16 -> {N, K, batch}, box {64, 64, 1}
-static int make_mnmajor_map(CUtensorMap* map, const void* base, int K, int N, int batch) {
-  const cuuint64_t dims[3] = {(cuuint64_t)N, (cuuint64_t)K, (cuuint64_t)batch};
-  const cuuint64_t strides[2] = {(cuuint64_t)N * 2, (cuuint64_t)K * N * 2};
-  const cuuint32_t box[3] = {64, 64, 1};
-  const cuuint32_t es[3] = {1, 1, 1};
-  return encode_tiled_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, es,
-                          CU_TENSOR_MAP_SWIZZLE_128B);
-}
-
 template <int EPI, bool B_MN>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, dim3 grid, cudaStream_t s) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(tile_gemm_kernel<EPI, B_MN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGSmem);
-    if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(tile_gemm)");
-    attr_set = true;
-  }
+  if (int rc = allow_dynamic_smem((const void*)tile_gemm_kernel<EPI, B_MN>, kGSmem, "tile_gemm")) return rc;
   tile_gemm_kernel<EPI, B_MN><<<grid, kGThreads, kGSmem, s>>>(ta, tb, p);
   static const char* const kEpiNames[] = {"EPI_STORE", "EPI_GRAM_SIGN", "EPI_GMFLOW"};
   return check_launchf("tile_gemm_kernel<%s,%d>", kEpiNames[EPI], (int)B_MN);
@@ -317,7 +293,7 @@ extern "C" int fresco_gram_sign(const void* xhat, const float* target, void* tsi
   if (batch <= 0 || tokens <= 0 || channels <= 0 || channels % 8 != 0 || tokens % 8 != 0)
     return set_error(FRESCO_ERR_ARG, "fresco_gram_sign: tokens and channels must be multiples of 8");
   CUtensorMap ta;
-  if (make_kmajor_map(&ta, xhat, tokens, channels, batch)) return FRESCO_ERR_TENSORMAP;
+  if (make_kmajor_map(&ta, xhat, tokens, channels, batch, 128)) return FRESCO_ERR_TENSORMAP;
   GemmParams p = {};
   p.M = tokens;
   p.N = tokens;
@@ -351,7 +327,7 @@ extern "C" int fresco_gram_grad(const void* tsign, const void* xhat, const float
     rc = fresco_gram_tx(tsign, xhat, static_cast<float*>(workspace), batch, tokens, channels, alpha, stream);
   } else {
     CUtensorMap ta, tb;
-    if (make_kmajor_map(&ta, tsign, tokens, tokens, batch)) return FRESCO_ERR_TENSORMAP;
+    if (make_kmajor_map(&ta, tsign, tokens, tokens, batch, 128)) return FRESCO_ERR_TENSORMAP;
     if (make_mnmajor_map(&tb, xhat, tokens, channels, batch)) return FRESCO_ERR_TENSORMAP;
     GemmParams p = {};
     p.M = tokens;
@@ -394,8 +370,8 @@ extern "C" int gmflow_global_corr_softmax(const float* feature0, const float* fe
   rc = check_launch("to_token_major_f16_kernel");
   if (rc) return rc;
   CUtensorMap m0, m1;
-  if (make_kmajor_map(&m0, t0, L, channels, batch)) return FRESCO_ERR_TENSORMAP;
-  if (make_kmajor_map(&m1, t1, L, channels, batch)) return FRESCO_ERR_TENSORMAP;
+  if (make_kmajor_map(&m0, t0, L, channels, batch, 128)) return FRESCO_ERR_TENSORMAP;
+  if (make_kmajor_map(&m1, t1, L, channels, batch, 128)) return FRESCO_ERR_TENSORMAP;
   GemmParams p = {};
   p.M = L;
   p.N = L;
@@ -421,8 +397,8 @@ extern "C" int gmflow_flow_attention(const void* q, const void* k, const float* 
   if (batch <= 0 || tokens <= 0 || channels <= 0 || channels % 8 != 0 || softmax_scale <= 0.f)
     return set_error(FRESCO_ERR_ARG, "gmflow_flow_attention: bad shape (channels must be a multiple of 8)");
   CUtensorMap mq, mk;
-  if (make_kmajor_map(&mq, q, tokens, channels, batch)) return FRESCO_ERR_TENSORMAP;
-  if (make_kmajor_map(&mk, k, tokens, channels, batch)) return FRESCO_ERR_TENSORMAP;
+  if (make_kmajor_map(&mq, q, tokens, channels, batch, 128)) return FRESCO_ERR_TENSORMAP;
+  if (make_kmajor_map(&mk, k, tokens, channels, batch, 128)) return FRESCO_ERR_TENSORMAP;
   GemmParams p = {};
   p.M = tokens;
   p.N = tokens;

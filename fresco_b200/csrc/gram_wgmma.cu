@@ -198,34 +198,10 @@ gram2_kernel(const __grid_constant__ CUtensorMap tm_a0, const __grid_constant__ 
   }
 }
 
-// K-major operand [batch, rows, K] fp16 -> {K, rows, batch}, box {64, box_rows, 1}
-static int make_kmajor_map2(CUtensorMap* map, const void* base, int rows, int K, int batch, int box_rows) {
-  const cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)rows, (cuuint64_t)batch};
-  const cuuint64_t strides[2] = {(cuuint64_t)K * 2, (cuuint64_t)rows * K * 2};
-  const cuuint32_t box[3] = {64, (cuuint32_t)box_rows, 1};
-  const cuuint32_t es[3] = {1, 1, 1};
-  return encode_tiled_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, es,
-                          CU_TENSOR_MAP_SWIZZLE_128B);
-}
-// MN-major B operand [batch, K rows, N cols] fp16 -> {N, K, batch}, box {64, 64, 1}
-static int make_mnmajor_map2(CUtensorMap* map, const void* base, int K, int N, int batch) {
-  const cuuint64_t dims[3] = {(cuuint64_t)N, (cuuint64_t)K, (cuuint64_t)batch};
-  const cuuint64_t strides[2] = {(cuuint64_t)N * 2, (cuuint64_t)K * N * 2};
-  const cuuint32_t box[3] = {64, 64, 1};
-  const cuuint32_t es[3] = {1, 1, 1};
-  return encode_tiled_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, es,
-                          CU_TENSOR_MAP_SWIZZLE_128B);
-}
-
 template <int MODE>
 static int launch_gram2(const CUtensorMap& a0, const CUtensorMap& b0, const CUtensorMap& a1, const CUtensorMap& b1,
                         const Gram2Params& p, cudaStream_t s) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gram2_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kG2Smem);
-    if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(gram2)");
-    attr_set = true;
-  }
+  if (int rc = allow_dynamic_smem((const void*)gram2_kernel<MODE>, kG2Smem, "gram2")) return rc;
   int grid = sm_count();
   if (grid > p.n_tiles) grid = p.n_tiles;
   gram2_kernel<MODE><<<grid, kG2Threads, kG2Smem, s>>>(a0, b0, a1, b1, p);
@@ -242,10 +218,10 @@ extern "C" int fresco_gram_sign_ref(const void* xhat, const void* yhat, void* ts
   if (batch <= 0 || tokens <= 0 || channels <= 0 || channels % 8 != 0 || tokens % 8 != 0)
     return set_error(FRESCO_ERR_ARG, "fresco_gram_sign_ref: tokens and channels must be multiples of 8");
   CUtensorMap ax, bx, ay, by;
-  if (make_kmajor_map2(&ax, xhat, tokens, channels, batch, 128)) return FRESCO_ERR_TENSORMAP;
-  if (make_kmajor_map2(&bx, xhat, tokens, channels, batch, 256)) return FRESCO_ERR_TENSORMAP;
-  if (make_kmajor_map2(&ay, yhat, tokens, channels, batch, 128)) return FRESCO_ERR_TENSORMAP;
-  if (make_kmajor_map2(&by, yhat, tokens, channels, batch, 256)) return FRESCO_ERR_TENSORMAP;
+  if (make_kmajor_map(&ax, xhat, tokens, channels, batch, 128)) return FRESCO_ERR_TENSORMAP;
+  if (make_kmajor_map(&bx, xhat, tokens, channels, batch, 256)) return FRESCO_ERR_TENSORMAP;
+  if (make_kmajor_map(&ay, yhat, tokens, channels, batch, 128)) return FRESCO_ERR_TENSORMAP;
+  if (make_kmajor_map(&by, yhat, tokens, channels, batch, 256)) return FRESCO_ERR_TENSORMAP;
   Gram2Params p = {};
   p.M = tokens;
   p.C = channels;
@@ -268,8 +244,8 @@ extern "C" int fresco_gram_tx(const void* tsign, const void* xhat, float* ghat, 
   if (batch <= 0 || tokens <= 0 || channels <= 0 || channels % 8 != 0 || tokens % 8 != 0)
     return set_error(FRESCO_ERR_ARG, "fresco_gram_tx: tokens and channels must be multiples of 8");
   CUtensorMap ta, tb;
-  if (make_kmajor_map2(&ta, tsign, tokens, tokens, batch, 128)) return FRESCO_ERR_TENSORMAP;
-  if (make_mnmajor_map2(&tb, xhat, tokens, channels, batch)) return FRESCO_ERR_TENSORMAP;
+  if (make_kmajor_map(&ta, tsign, tokens, tokens, batch, 128)) return FRESCO_ERR_TENSORMAP;
+  if (make_mnmajor_map(&tb, xhat, tokens, channels, batch)) return FRESCO_ERR_TENSORMAP;
   Gram2Params p = {};
   p.M = tokens;
   p.C = channels;

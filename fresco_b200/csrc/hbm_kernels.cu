@@ -386,61 +386,10 @@ __device__ __forceinline__ void st_from_float<float>(float* p, float v) { *p = v
 template <>
 __device__ __forceinline__ void st_from_float<__half>(__half* p, float v) { *p = __float2half_rn(v); }
 
-// one CTA per (chunk, channel): the running plane lives in shared memory (fp32, like the
-// reference's `latent = sample.to(float32)`), so the N-1 dependent blends are block-local.
-template <typename T>
-__global__ void warp_chain_smem_kernel(const T* __restrict__ sample, T* __restrict__ out,
-                                       const float* __restrict__ bwd_flow, const float* __restrict__ fwd_flow_last,
-                                       const float* __restrict__ blend, int frames, int channels, int h, int w) {
-  extern __shared__ float planes[];
-  const int hw = h * w;
-  float* cur = planes;
-  float* nxt = planes + hw;
-  const int c = blockIdx.x % channels;
-  const int j = blockIdx.x / channels;
-  auto plane_of = [&](int f) { return ((long long)(j * frames + f) * channels + c) * hw; };
-
-  for (int i = threadIdx.x; i < hw; i += blockDim.x) {
-    const float v = ld_as_float(sample + plane_of(0) + i);
-    cur[i] = v;
-    st_from_float(out + plane_of(0) + i, v);
-  }
-  __syncthreads();
-  for (int ii = 0; ii + 1 < frames; ++ii) {
-    const float* fl = bwd_flow + (long long)ii * 2 * hw;
-    const float* mk = blend + (long long)ii * hw;
-    const bool last = (ii + 2 == frames);
-#pragma unroll 4
-    for (int i = threadIdx.x; i < hw; i += blockDim.x) {
-      const int x = i % w, y = i / w;
-      const Taps tp = make_taps(x + fl[i], y + fl[hw + i], h, w);
-      const float m = mk[i];
-      const float z = ld_as_float(sample + plane_of(ii + 1) + i);
-      const float v = z * (1.f - m) + sample_taps(cur, tp) * m;
-      nxt[i] = v;
-      if (!last) st_from_float(out + plane_of(ii + 1) + i, v);
-    }
-    __syncthreads();
-    float* t = cur;
-    cur = nxt;
-    nxt = t;
-  }
-  // closing blend: frame N-1 <- warp(frame 0, fwd_flow[N-1])  (flow_utils.py:47-51)
-  for (int i = threadIdx.x; i < hw; i += blockDim.x) nxt[i] = ld_as_float(sample + plane_of(0) + i);
-  __syncthreads();
-  const float* mk = blend + (long long)(frames - 1) * hw;
-  for (int i = threadIdx.x; i < hw; i += blockDim.x) {
-    const int x = i % w, y = i / w;
-    const Taps tp = make_taps(x + fwd_flow_last[i], y + fwd_flow_last[hw + i], h, w);
-    const float m = mk[i];
-    const float v = cur[i] * (1.f - m) + sample_taps(nxt, tp) * m;
-    st_from_float(out + plane_of(frames - 1) + i, v);
-  }
-}
-
-// Channel-grouped variant: the per-pixel work that does not depend on the channel (two flow loads, the four bilinear
-// taps, the blend weight) is done ONCE per pixel and applied to K planes; K (chunk, channel) planes per CTA keep their
-// running frames in shared memory.  Same arithmetic, same order of operations per element as the kernel above.
+// K (chunk, channel) planes per CTA keep their running frames in shared memory (fp32, like the reference's
+// `latent = sample.to(float32)`), so the N-1 dependent blends are block-local.  The per-pixel work that does not
+// depend on the channel (two flow loads, the four bilinear taps, the blend weight) is done ONCE per pixel and applied
+// to the K planes.
 template <typename T, int K>
 __global__ void __launch_bounds__(512)
 warp_chain_group_kernel(const T* __restrict__ sample, T* __restrict__ out, const float* __restrict__ bwd_flow,
@@ -534,7 +483,7 @@ __device__ __forceinline__ float4 sample_taps4(const float4* plane, const Taps& 
 // Channel-QUAD variant (the one warp_tensor runs on decoder features; see warp_loss_quad_kernel below for the
 // measurement behind it): NQ quads of four (chunk, channel) planes per CTA, interleaved per pixel as float4 in shared
 // memory, so the flows / blend weight of a pixel are fetched and its taps built once for 4 NQ channels and one 16-byte
-// shared load serves a tap for four of them.  Same arithmetic per element as the kernels above.
+// shared load serves a tap for four of them.  Same arithmetic per element as warp_chain_group_kernel.
 template <typename T, int P, int NQ>
 __global__ void __launch_bounds__(1024, 1)
 warp_chain_quad_kernel(const T* __restrict__ sample, T* __restrict__ out, const float* __restrict__ bwd_flow,
@@ -1535,13 +1484,7 @@ static int launch_temporal_rows(const void* q_raw, const void* k_raw, const void
   const size_t smem = tpb * per_traj;
   if (smem > 200 * 1024) return FRESCO_ERR_UNSUPPORTED;
   int threads = (tpb * rows_per_traj + 31) / 32 * 32;
-  static size_t attr_smem = 0;
-  if (smem > 48 * 1024 && smem > attr_smem) {
-    cudaError_t e = cudaFuncSetAttribute(temporal_attn_rows_kernel<D, NMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)smem);
-    if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(temporal_attn_rows)");
-    attr_smem = smem;
-  }
+  if (int rc = allow_dynamic_smem((const void*)temporal_attn_rows_kernel<D, NMAX>, smem, "temporal_attn_rows")) return rc;
   const int blocks = chunks * ((tokens + tpb - 1) / tpb);
   temporal_attn_rows_kernel<D, NMAX><<<blocks, threads, smem, s>>>(
       (const __half*)q_raw, (const __half*)k_raw, (const __half*)v_src, (__half*)out, fwd_map, traj_mask, frames, tokens,
@@ -1588,10 +1531,7 @@ extern "C" int fresco_temporal_attn_fwd_strided(const void* q_raw, const void* k
       (((size_t)3 * frames * head_dim * sizeof(__half) + (size_t)frames * frames * sizeof(float)) + 15) & ~size_t(15);
   const size_t smem = per_warp * heads;
   if (smem > 200 * 1024) return set_error(FRESCO_ERR_UNSUPPORTED, "fresco_temporal_attn_fwd: frames*head_dim too large");
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(temporal_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(temporal_attn)");
-  }
+  if (int rc = allow_dynamic_smem((const void*)temporal_attn_kernel, smem, "temporal_attn")) return rc;
   temporal_attn_kernel<<<chunks * tokens, 32 * heads, smem, s>>>(
       (const __half*)q_raw, (const __half*)k_raw, (const __half*)v_src, (__half*)out, fwd_map, traj_mask, frames,
       tokens, heads, head_dim, scale);
@@ -1612,13 +1552,7 @@ template <typename T, int K>
 static int launch_chain_group(const void* sample, void* out, const float* bwd_flow, const float* fwd_flow_last,
                               const float* blend, int chunks, int frames, int channels, int h, int w, cudaStream_t s) {
   const size_t smem = (size_t)2 * K * h * w * sizeof(float);
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(warp_chain_group_kernel<T, K>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         200 * 1024);
-    if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(warp_chain_group)");
-    attr_set = true;
-  }
+  if (int rc = allow_dynamic_smem((const void*)warp_chain_group_kernel<T, K>, 200 * 1024, "warp_chain_group")) return rc;
   const int planes = chunks * channels;
   warp_chain_group_kernel<T, K><<<(planes + K - 1) / K, 512, smem, s>>>((const T*)sample, (T*)out, bwd_flow, fwd_flow_last,
                                                                        blend, frames, channels, planes, h, w);
@@ -1626,20 +1560,17 @@ static int launch_chain_group(const void* sample, void* out, const float* bwd_fl
 }
 
 // (P pixels per thread, NQ channel quads per CTA) for a plane of hw pixels: as many quads as shared memory (bytes_per_px
-// per quad, 200 KB) and the divisibility of the channel count allow, at most 4 values per thread to carry, threads <= 1024
+// per quad, 200 KB) and the divisibility of the channel count allow, P * NQ == 4 carried float4 per thread, so one of
+// (1,4), (2,2), (4,1).  False when that needs more than 1024 threads: the caller takes its channel-grouped kernel.
 static bool quad_config(int hw, int channels, int planes, int bytes_per_px, int& P, int& NQ, int& T) {
   if (channels % 4 != 0) return false;
   for (NQ = 4; NQ >= 1; NQ >>= 1) {
     if (channels % (4 * NQ) != 0) continue;
     if ((size_t)NQ * hw * bytes_per_px > 200 * 1024) continue;
     if (NQ > 1 && planes / (4 * NQ) < sm_count()) continue;           // keep every SM busy
-    P = 4 / NQ;                                                       // P * NQ == 4 carried float4 per thread
+    P = 4 / NQ;
     T = ((hw + P - 1) / P + 31) / 32 * 32;
-    while (T > 1024 && P * NQ < 4 * 4) {                              // large planes: more pixels per thread
-      P *= 2;
-      T = ((hw + P - 1) / P + 31) / 32 * 32;
-    }
-    if (T > 1024 || P > 4) continue;
+    if (T > 1024) return false;
     if (T < 32) T = 32;
     return true;
   }
@@ -1651,13 +1582,7 @@ static int launch_chain_quad(const void* sample, void* out, const float* bwd_flo
                              const float* blend, int chunks, int frames, int channels, int h, int w, int threads,
                              cudaStream_t s) {
   const size_t smem = (size_t)NQ * h * w * 32;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(warp_chain_quad_kernel<T, P, NQ>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         200 * 1024);
-    if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(warp_chain_quad)");
-    attr_set = true;
-  }
+  if (int rc = allow_dynamic_smem((const void*)warp_chain_quad_kernel<T, P, NQ>, 200 * 1024, "warp_chain_quad")) return rc;
   warp_chain_quad_kernel<T, P, NQ><<<chunks * channels / (4 * NQ), threads, smem, s>>>(
       (const T*)sample, (T*)out, bwd_flow, fwd_flow_last, blend, frames, channels, h, w);
   return check_launchf("warp_chain_quad_kernel<%s,%d,%d>", sizeof(T) == 2 ? "half" : "float", P, NQ);
@@ -1673,7 +1598,7 @@ static int launch_chain(const void* sample, void* out, const float* bwd_flow, co
   if (P == PP && NQ == QQ)                                                                                             \
     return launch_chain_quad<T, PP, QQ>(sample, out, bwd_flow, fwd_flow_last, blend, chunks, frames, channels, h, w,   \
                                         threads, s);
-    CQ(1, 4) CQ(2, 2) CQ(4, 1) CQ(1, 2) CQ(2, 1) CQ(1, 1)
+    CQ(1, 4) CQ(2, 2) CQ(4, 1)
 #undef CQ
   }
   // planes per CTA: as many as keep two CTAs on an SM (<= ~100 KB of shared memory each) and the grid above two waves
@@ -1763,19 +1688,14 @@ extern "C" int fresco_warp_loss_fwd_bwd_halo(const float* cs, const float* fwd_f
       const int grid_q = chunks * channels / (4 * NQ);
 #define LQ(PP, QQ)                                                                                                      \
   if (P == PP && NQ == QQ) {                                                                                            \
-    static bool attr_set = false;                                                                                       \
-    if (!attr_set) {                                                                                                    \
-      cudaError_t e = cudaFuncSetAttribute(warp_loss_quad_kernel<PP, QQ>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
-                                           200 * 1024);                                                                 \
-      if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(warp_loss_quad)");                           \
-      attr_set = true;                                                                                                  \
-    }                                                                                                                   \
+    if (int rc = allow_dynamic_smem((const void*)warp_loss_quad_kernel<PP, QQ>, 200 * 1024, "warp_loss_quad"))         \
+      return rc;                                                                                                        \
     warp_loss_quad_kernel<PP, QQ><<<grid_q, threads, smem_q, s>>>(                                                      \
         cs, fwd_flow, bwd_flow, fwd_keep, bwd_keep, (const uint4*)bwd_ell, (const uint4*)fwd_ell, overflow, n_overflow, \
         grad, loss_acc, accumulate, frames, channels, h, w, kk, halo_cs, halo_grad);                                    \
     return check_launchf("warp_loss_quad_kernel<%d,%d>", PP, QQ);                                                       \
   }
-      LQ(1, 4) LQ(2, 2) LQ(4, 1) LQ(1, 2) LQ(2, 1) LQ(1, 1)
+      LQ(1, 4) LQ(2, 2) LQ(4, 1)
 #undef LQ
     }
   }
@@ -1800,13 +1720,8 @@ extern "C" int fresco_warp_loss_fwd_bwd_halo(const float* cs, const float* fwd_f
       const int grid = (planes + K - 1) / K;
 #define LOSS_CASE(PP, KK)                                                                                               \
   if (P == PP && KT == KK) {                                                                                            \
-    static bool attr_set = false;                                                                                       \
-    if (!attr_set) {                                                                                                    \
-      cudaError_t e = cudaFuncSetAttribute(warp_loss_group_kernel<PP, KK>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                           200 * 1024);                                                                 \
-      if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(warp_loss_group)");                          \
-      attr_set = true;                                                                                                  \
-    }                                                                                                                   \
+    rc = allow_dynamic_smem((const void*)warp_loss_group_kernel<PP, KK>, 200 * 1024, "warp_loss_group");               \
+    if (rc) return rc;                                                                                                  \
     warp_loss_group_kernel<PP, KK><<<grid, T, smem, s>>>(cs, fwd_flow, bwd_flow, fwd_keep, bwd_keep,                    \
                                                          (const uint4*)bwd_ell, (const uint4*)fwd_ell, overflow,        \
                                                          n_overflow, grad, loss_acc, accumulate, frames, channels,      \
@@ -1827,12 +1742,7 @@ extern "C" int fresco_warp_loss_fwd_bwd_halo(const float* cs, const float* fwd_f
   // ---- any other plane size: one CTA per plane (round-1 kernel)
   const size_t smem = (size_t)4 * h * w * sizeof(float);
   if (smem > 200 * 1024) return set_error(FRESCO_ERR_UNSUPPORTED, "fresco_warp_loss_fwd_bwd: plane too large for shared memory");
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(warp_loss_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(warp_loss)");
-    attr_set = true;
-  }
+  if (int rc = allow_dynamic_smem((const void*)warp_loss_kernel, 200 * 1024, "warp_loss")) return rc;
   warp_loss_kernel<<<chunks * channels, 256, smem, s>>>(
       cs, fwd_flow, bwd_flow, fwd_keep, bwd_keep, (const uint4*)bwd_ell, (const uint4*)fwd_ell, overflow, n_overflow,
       grad, loss_acc, accumulate, frames, channels, h, w, kk, halo_cs, halo_grad);

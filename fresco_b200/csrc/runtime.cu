@@ -1,9 +1,12 @@
-// Error state, launch accounting and the driver-API entry point for TMA tensor maps.
+// Error state, launch accounting, TMA tensor maps and per-device launch set-up.
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
+#include <mutex>
+#include <utility>
 
 #include "fresco_internal.h"
 
@@ -77,6 +80,46 @@ int encode_tiled_map(CUtensorMap* map, CUtensorMapDataType dtype, int rank, void
   return FRESCO_OK;
 }
 
+int make_kmajor_map(CUtensorMap* map, const void* base, int rows, int K, int batch, int box_rows) {
+  const cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)rows, (cuuint64_t)batch};
+  const cuuint64_t strides[2] = {(cuuint64_t)K * 2, (cuuint64_t)rows * K * 2};
+  const cuuint32_t box[3] = {64, (cuuint32_t)box_rows, 1};
+  const cuuint32_t es[3] = {1, 1, 1};
+  return encode_tiled_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, es,
+                          CU_TENSOR_MAP_SWIZZLE_128B);
+}
+
+int make_mnmajor_map(CUtensorMap* map, const void* base, int K, int N, int batch) {
+  const cuuint64_t dims[3] = {(cuuint64_t)N, (cuuint64_t)K, (cuuint64_t)batch};
+  const cuuint64_t strides[2] = {(cuuint64_t)N * 2, (cuuint64_t)K * N * 2};
+  const cuuint32_t box[3] = {64, 64, 1};
+  const cuuint32_t es[3] = {1, 1, 1};
+  return encode_tiled_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, es,
+                          CU_TENSOR_MAP_SWIZZLE_128B);
+}
+
+// per-device state: the dynamic shared memory each kernel may use, and the SM count
+static std::mutex g_device_mu;
+static std::map<std::pair<const void*, int>, size_t> g_smem_allowed;
+static std::map<int, int> g_sm_count;
+
+int allow_dynamic_smem(const void* kernel, size_t bytes, const char* what) {
+  if (bytes <= 48 * 1024) return FRESCO_OK;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  std::lock_guard<std::mutex> lock(g_device_mu);
+  size_t& allowed = g_smem_allowed[{kernel, dev}];
+  if (bytes <= allowed) return FRESCO_OK;
+  const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  if (e != cudaSuccess) {
+    char where[128];
+    snprintf(where, sizeof(where), "cudaFuncSetAttribute(%s)", what);
+    return set_cuda_error(e, where);
+  }
+  allowed = bytes;
+  return FRESCO_OK;
+}
+
 static const char* const kOptionNames[OPT_COUNT] = {"FRESCO_ATTN_WIDE", "FRESCO_ATTN_POLY", "FRESCO_ATTN_ROWSUM",
                                                     "FRESCO_TEMPORAL_V", "FRESCO_GRAM_V"};
 static std::atomic<int> g_opt_state[OPT_COUNT];      // 0 = not looked at, 1 = unset (use the default), 2 = set
@@ -94,10 +137,11 @@ int option(Option which, int dflt) {
 }
 
 int sm_count() {
-  static int n = 0;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  std::lock_guard<std::mutex> lock(g_device_mu);
+  int& n = g_sm_count[dev];
   if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     if (n <= 0) n = 148;
   }
