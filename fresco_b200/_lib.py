@@ -45,6 +45,9 @@ _SIGNATURES = {
     "fresco_gram_grad_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "fresco_gram_sign_ref": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_float, _P]),
     "fresco_gram_tx": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_float, _P]),
+    "fresco_gram_sign_scaled": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_double, _P]),
+    "fresco_gram_sign_ref_scaled": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_double, _P]),
+    "fresco_gram_grad_scaled": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_double, _P, c_size_t, _P]),
     "fresco_adam_step": (c_int, [_P, _P, _P, _P, c_longlong, c_int, c_double, c_double, c_double, c_double, _P]),
     "fresco_adain": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P]),
     "gmflow_global_corr_softmax": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, c_size_t, _P]),

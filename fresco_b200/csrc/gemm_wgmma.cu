@@ -287,8 +287,8 @@ __global__ void to_token_major_f16_kernel(const float* __restrict__ src, __half*
 
 using namespace fresco;
 
-extern "C" int fresco_gram_sign(const void* xhat, const float* target, void* tsign, float* loss_acc, int batch,
-                                int tokens, int channels, float weight, void* stream) {
+extern "C" int fresco_gram_sign_scaled(const void* xhat, const float* target, void* tsign, float* loss_acc, int batch,
+                                       int tokens, int channels, double scale, void* stream) {
   if (!xhat || !target || !tsign) return set_error(FRESCO_ERR_ARG, "fresco_gram_sign: null pointer");
   if (batch <= 0 || tokens <= 0 || channels <= 0 || channels % 8 != 0 || tokens % 8 != 0)
     return set_error(FRESCO_ERR_ARG, "fresco_gram_sign: tokens and channels must be multiples of 8");
@@ -302,25 +302,31 @@ extern "C" int fresco_gram_sign(const void* xhat, const float* target, void* tsi
   p.target = target;
   p.tsign = static_cast<__half*>(tsign);
   p.loss_acc = loss_acc;
-  p.loss_scale = (float)((double)weight / ((double)batch * tokens * tokens));
+  p.loss_scale = (float)scale;
   const int tiles = (tokens + 127) / 128;
   return launch_gemm<EPI_GRAM_SIGN, false>(ta, ta, p, dim3(tiles, tiles, batch), (cudaStream_t)stream);
+}
+
+extern "C" int fresco_gram_sign(const void* xhat, const float* target, void* tsign, float* loss_acc, int batch,
+                                int tokens, int channels, float weight, void* stream) {
+  return fresco_gram_sign_scaled(xhat, target, tsign, loss_acc, batch, tokens, channels,
+                                 (double)weight / ((double)batch * tokens * tokens), stream);
 }
 
 extern "C" size_t fresco_gram_grad_workspace_bytes(int batch, int tokens, int channels) {
   return (size_t)batch * tokens * channels * sizeof(float);
 }
 
-extern "C" int fresco_gram_grad(const void* tsign, const void* xhat, const float* norms, float* grad, int batch,
-                                int tokens, int channels, float weight, void* workspace, size_t workspace_bytes,
-                                void* stream) {
+extern "C" int fresco_gram_grad_scaled(const void* tsign, const void* xhat, const float* norms, float* grad, int batch,
+                                       int tokens, int channels, double scale, void* workspace, size_t workspace_bytes,
+                                       void* stream) {
   if (!tsign || !xhat || !norms || !grad || !workspace) return set_error(FRESCO_ERR_ARG, "fresco_gram_grad: null pointer");
   if (batch <= 0 || tokens <= 0 || channels <= 0 || channels % 8 != 0 || tokens % 8 != 0)
     return set_error(FRESCO_ERR_ARG, "fresco_gram_grad: tokens and channels must be multiples of 8");
   if (workspace_bytes < fresco_gram_grad_workspace_bytes(batch, tokens, channels))
     return set_error(FRESCO_ERR_ARG, "fresco_gram_grad: workspace too small");
   cudaStream_t s = (cudaStream_t)stream;
-  const float alpha = (float)((double)weight / ((double)batch * tokens * tokens));
+  const float alpha = (float)scale;
   int rc;
   if (option(OPT_GRAM_V, 2) == 2) {
     // persistent 128 x 256 tiles (gram_wgmma.cu)
@@ -343,6 +349,13 @@ extern "C" int fresco_gram_grad(const void* tsign, const void* xhat, const float
   gram_project_kernel<<<batch * tiles, 256, 0, s>>>(static_cast<const float*>(workspace), (const __half*)xhat, norms,
                                                     grad, channels, tokens);
   return check_launch("gram_project_kernel");
+}
+
+extern "C" int fresco_gram_grad(const void* tsign, const void* xhat, const float* norms, float* grad, int batch,
+                                int tokens, int channels, float weight, void* workspace, size_t workspace_bytes,
+                                void* stream) {
+  return fresco_gram_grad_scaled(tsign, xhat, norms, grad, batch, tokens, channels,
+                                 (double)weight / ((double)batch * tokens * tokens), workspace, workspace_bytes, stream);
 }
 
 extern "C" size_t fresco_gmflow_corr_workspace_bytes(int batch, int channels, int h, int w) {

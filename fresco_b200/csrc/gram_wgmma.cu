@@ -36,7 +36,7 @@ struct Gram2Params {
   // G2_SIGN
   __half* tsign;              // [batch, M, M]
   float* loss_acc;
-  float loss_scale;           // weight / (batch * M * M)
+  float loss_scale;           // weight / (batch * M * M), rounded once
   // G2_GRAD
   float* out;                 // [batch, M, C]
   float alpha;
@@ -212,8 +212,8 @@ static int launch_gram2(const CUtensorMap& a0, const CUtensorMap& b0, const CUte
 
 using namespace fresco;
 
-extern "C" int fresco_gram_sign_ref(const void* xhat, const void* yhat, void* tsign, float* loss_acc, int batch,
-                                    int tokens, int channels, float weight, void* stream) {
+extern "C" int fresco_gram_sign_ref_scaled(const void* xhat, const void* yhat, void* tsign, float* loss_acc, int batch,
+                                           int tokens, int channels, double scale, void* stream) {
   if (!xhat || !yhat || !tsign) return set_error(FRESCO_ERR_ARG, "fresco_gram_sign_ref: null pointer");
   if (batch <= 0 || tokens <= 0 || channels <= 0 || channels % 8 != 0 || tokens % 8 != 0)
     return set_error(FRESCO_ERR_ARG, "fresco_gram_sign_ref: tokens and channels must be multiples of 8");
@@ -234,8 +234,14 @@ extern "C" int fresco_gram_sign_ref(const void* xhat, const void* yhat, void* ts
   p.n_tiles = per * batch;
   p.tsign = static_cast<__half*>(tsign);
   p.loss_acc = loss_acc;
-  p.loss_scale = (float)((double)weight / ((double)batch * tokens * tokens));
+  p.loss_scale = (float)scale;
   return launch_gram2<G2_SIGN>(ax, bx, ay, by, p, (cudaStream_t)stream);
+}
+
+extern "C" int fresco_gram_sign_ref(const void* xhat, const void* yhat, void* tsign, float* loss_acc, int batch,
+                                    int tokens, int channels, float weight, void* stream) {
+  return fresco_gram_sign_ref_scaled(xhat, yhat, tsign, loss_acc, batch, tokens, channels,
+                                     (double)weight / ((double)batch * tokens * tokens), stream);
 }
 
 extern "C" int fresco_gram_tx(const void* tsign, const void* xhat, float* ghat, int batch, int tokens, int channels,

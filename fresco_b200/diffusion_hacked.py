@@ -414,8 +414,10 @@ def optimize_feature(sample, flows, occs, correlation_matrix=[], intra_weight=1e
     same per-batch parameters).  The spatial term, Adam and AdaIN are per frame.  The temporal term couples frame f with
     frame f+1 of the ring (:444): per Adam iteration every rank receives the following rank's first frame as a halo,
     evaluates its own pairs in the open-chain form and sends the halo's gradient on (two neighbour exchanges of
-    [chunks, C, h, w] fp32 per iteration).  The result is bit-identical to the unsharded call when the ranks hold a
-    power-of-two share of the frames (the loss weights stay exact)."""
+    [chunks, C, h, w] fp32 per iteration).  The ranks hold the ``frame_range`` blocks of the batch, which need not be
+    even; the batch frame count is that of ``flows`` (without flows: one all-reduce of the local counts).  The result
+    is bit-identical to the unsharded call: the loss means run over the whole batch and the Gram kernels get the same
+    fp32 loss scale as unsharded (``ops.gram_*`` divide the rank's share of the weight in double and round once)."""
     have_temporal = flows is not None and occs is not None and optimize_temporal
     if (not have_temporal) and (intra_weight == 0 or len(correlation_matrix) == 0):
         return sample
@@ -430,11 +432,16 @@ def optimize_feature(sample, flows, occs, correlation_matrix=[], intra_weight=1e
         rank = int(shard[1])
         third = shard[2] if len(shard) > 2 else None
         comm = third if hasattr(third, "shift") else RingComm(world, rank, third)
-        total = n * world
-        if have_temporal and flows[0].shape[0] != total:
-            raise FrescoError("optimize_feature: flows must cover the whole batch (%d frames), got %d"
-                              % (total, flows[0].shape[0]))
-        lo = frame_range(total, world, rank)[0]
+        if flows is not None:
+            total = int(flows[0].shape[0])
+        else:
+            count = torch.full((1,), n, dtype=torch.int64, device=sample.device)
+            comm.all_reduce_sum(count)
+            total = int(count.item())
+        lo, hi = frame_range(total, world, rank)
+        if hi - lo != n:
+            raise FrescoError("optimize_feature: rank %d of %d owns frames [%d, %d) of the %d-frame batch, got %d"
+                              % (rank, world, lo, hi, total, n))
     cs = sample.to(torch.float32).reshape(unet_chunk_size, n, C, h, w).contiguous().clone()
     grad = torch.empty_like(cs)
     exp_avg = torch.zeros_like(cs)
@@ -452,7 +459,8 @@ def optimize_feature(sample, flows, occs, correlation_matrix=[], intra_weight=1e
     spatial = target is not None and intra_weight > 0
     if spatial and not isinstance(target, GramTarget):
         target = target.to(torch.float32).contiguous()
-    # F.l1_loss averages over the frames of the WHOLE batch: a rank's share of the weight (exact for power-of-two shares)
+    # F.l1_loss averages over the frames of the WHOLE batch: a rank's share of the weight, which the Gram kernels divide
+    # by this rank's batch in double (ops.gram_*), so the fp32 loss scale is the unsharded one
     weight = intra_weight * (float(n) / float(total))
     loss_acc = torch.zeros(1, dtype=torch.float32, device=sample.device) if trace is not None else None
     for it in range(1, iters + 1):
@@ -596,7 +604,7 @@ def get_intraframe_paras(pipe, imgs, frescoProc, prompt_embeds, do_classifier_fr
     decoder features.
 
     ``shard=(world, rank[, group])`` (not in the reference): ``imgs`` / ``prompt_embeds`` hold ALL N frames; the
-    initial noise is drawn for all of them from the seeded generator and this rank's frames [rank*N/G, (rank+1)*N/G)
+    initial noise is drawn for all of them from the seeded generator and this rank's frames [rank*N//G, (rank+1)*N//G)
     are sliced, encoded and run through the store pass.  The controller then holds this rank's reference inputs and
     the targets cover this rank's frames (both CFG chunks): what the sharded processor and
     ``optimize_feature(shard=...)`` take.  The pass is per frame, so no collective is issued."""
@@ -633,10 +641,10 @@ def get_flow_and_interframe_paras(flow_model, imgs, visualize_pipeline=False, sh
     redirected to fresco_b200.gmflow_matching, see INTEGRATION.md).
 
     ``shard=(world, rank[, group])`` (not in the reference): every rank gets all N frames, runs GMFlow on its own
-    pairs [rank*N/G, (rank+1)*N/G) only and one all-gather assembles the whole batch's flows (rank order == pair
-    order).  Occlusions, masks and trajectories are then built from the gathered flows on every rank, as unsharded:
+    pairs ``frame_range(N, world, rank)`` only and one all-gather (blocks padded to the largest share) assembles the
+    whole batch's flows (rank order == pair order).  Occlusions, masks and trajectories are then built from the gathered flows on every rank, as unsharded:
     the return values are the whole batch's, as in the unsharded call."""
-    from .dist import all_gather_blocks, shard_frames
+    from .dist import all_gather_frames, shard_frames
     from .flow_utils import flow_warp, forward_backward_consistency_check, get_mapping_ind
     dev = next(flow_model.parameters()).device
     images = torch.stack([torch.from_numpy(im).permute(2, 0, 1).float() for im in imgs], dim=0).to(dev)
@@ -647,9 +655,7 @@ def get_flow_and_interframe_paras(flow_model, imgs, visualize_pipeline=False, sh
                      prop_radius_list=[-1], pred_bidir_flow=True)
     flow = res["flow_preds"][-1]                                        # [2 * pairs, 2, H, W]: forward | backward
     if shard is not None and shard[0] > 1:
-        world = shard[0]
-        gathered = all_gather_blocks(flow, world, shard[2] if len(shard) > 2 else None)
-        flow = gathered.view(world, 2, hi - lo, *flow.shape[1:]).transpose(0, 1).reshape(2 * len(images), *flow.shape[1:])
+        flow = all_gather_frames(flow, len(images), shard[0], 2, shard[2] if len(shard) > 2 else None)
     fwd_flows, bwd_flows = flow.chunk(2)
     fwd_flows, bwd_flows = fwd_flows.contiguous(), bwd_flows.contiguous()
     fwd_occs, bwd_occs = forward_backward_consistency_check(fwd_flows, bwd_flows)

@@ -1,8 +1,9 @@
 """Frame-sharded FRESCO attention for one multi-GPU box (NCCL over NVLink / NVSwitch).
 
 The reference has no collective on this path (SURVEY 2.1); this module is the multi-GPU design for BASELINE config 4: the
-N keyframes of ONE batch are split contiguously over G ranks (rank r owns frames [r*N/G, (r+1)*N/G) of both CFG
-chunks) and the UNet body runs as plain replicas.  Only FRESCO attention couples frames:
+N keyframes of ONE batch are split contiguously over G ranks (rank r owns frames ``frame_range(N, G, r)`` =
+[r*N//G, (r+1)*N//G) of both CFG chunks; G need not divide N) and the UNet body runs as plain replicas.  Only FRESCO
+attention couples frames:
 
 * cross-frame attention (src/diffusion_hacked.py:225-247, :303-305): every query frame attends the same K/V set = all
   tokens of frame 0 + the occluded tokens of frames 1..N-1.  Each rank compacts the selected rows of ITS frames straight
@@ -11,7 +12,7 @@ chunks) and the UNet body runs as plain replicas.  Only FRESCO attention couples
   padding, and the attention kernel reads K and V out of the interleaved buffer through strided TMA maps -- the
   reference's row-major (frame, token) order is kept because rank order == frame order.
 * temporal-guided attention (:320-367) mixes all N frames along each flow trajectory.  It is sharded by TRAJECTORY:
-  rank s owns trajectories [s*L/G, (s+1)*L/G); one all-to-all sends it the q | k | attention-output rows those
+  rank s owns trajectories ``frame_range(L, G, s)``; one all-to-all sends it the q | k | attention-output rows those
   trajectories visit in every rank's frames (1/G of the data instead of an all-gather of all of it), it runs the
   N x N attention for its trajectories only (1/G of the work instead of all of it on every rank), and a second
   all-to-all returns the result rows to the ranks that own the frames.
@@ -24,17 +25,25 @@ per-batch plans exist, so a whole UNet step (collectives included) can be captur
 from __future__ import annotations
 
 import math
-from typing import Optional, Tuple
+from typing import List, Optional, Tuple
 
 import torch
 import torch.distributed as dist
 
 
 def frame_range(n_frames: int, world: int, rank: int) -> Tuple[int, int]:
-    if n_frames % world != 0:
-        raise ValueError(f"{n_frames} frames do not split evenly over {world} ranks")
-    per = n_frames // world
-    return rank * per, (rank + 1) * per
+    """[lo, hi) = [rank*N//G, (rank+1)*N//G): the contiguous block of the N items (frames of a batch, trajectories of
+    the temporal exchange) rank ``rank`` of ``world`` owns.  Rank order is item order, every rank gets floor(N/G) or
+    ceil(N/G) items, and when G divides N this is the even split."""
+    if n_frames < world:
+        raise ValueError(f"{n_frames} frames cannot be split over {world} ranks (every rank needs at least one): run "
+                         f"the batch on a process group of {n_frames} ranks, shard=({n_frames}, rank, group)")
+    return rank * n_frames // world, (rank + 1) * n_frames // world
+
+
+def block_sizes(n_frames: int, world: int) -> List[int]:
+    """the share of every rank under ``frame_range``, in rank order"""
+    return [hi - lo for lo, hi in (frame_range(n_frames, world, r) for r in range(world))]
 
 
 def shard_frames(n_frames: int, shard) -> Tuple[int, int]:
@@ -57,6 +66,25 @@ def all_gather_blocks(t: torch.Tensor, world: int, group=None) -> torch.Tensor:
     out = torch.empty((world,) + tuple(t.shape), dtype=t.dtype, device=t.device)
     dist.all_gather_into_tensor(out.view(-1, *t.shape[1:]), t, group=group)
     return out
+
+
+def all_gather_frames(t: torch.Tensor, n_frames: int, world: int, chunks: int = 1, group=None) -> torch.Tensor:
+    """``[chunks * N, ...]``: the whole ``(chunk, frame)``-major batch from every rank's ``t = [chunks * n_r, ...]``
+    (its ``frame_range`` block of each chunk).  Every block is padded to the largest share, one all-gather moves them,
+    and the padding is dropped; the shares are host ints, so nothing reads from the device."""
+    sizes = block_sizes(n_frames, world)
+    per = max(sizes)
+    inner = tuple(t.shape[1:])
+    mine = t.shape[0] // chunks
+    if mine == per:
+        send = t
+    else:
+        send = torch.zeros((chunks, per) + inner, dtype=t.dtype, device=t.device)
+        send[:, :mine] = t.reshape((chunks, mine) + inner)
+    full = all_gather_blocks(send.reshape((chunks * per,) + inner), world, group).view((world, chunks, per) + inner)
+    if min(sizes) == per:
+        return full.transpose(0, 1).reshape((chunks * n_frames,) + inner)
+    return torch.cat([full[r, :, :sizes[r]] for r in range(world)], 1).reshape((chunks * n_frames,) + inner)
 
 
 class RingComm:
@@ -122,8 +150,7 @@ class ShardedKVExchange:
         self.world, self.rank, self.group, self.chunks = world, rank, group, chunks
         self.lo, self.hi = frame_range(n_frames, world, rank)
         per_frame = attn_mask.sum(1).tolist()                               # one host sync per batch and resolution
-        n_local = self.hi - self.lo
-        counts = [int(sum(per_frame[r * n_local:(r + 1) * n_local])) for r in range(world)]
+        counts = [int(sum(per_frame[lo:hi])) for lo, hi in (frame_range(n_frames, world, r) for r in range(world))]
         self.counts = counts
         self.max_count = max(max(counts), 1)
         self.total = sum(counts)
@@ -164,32 +191,39 @@ class ShardedTrajectoryExchange:
     """Per-batch plan of the trajectory-sharded temporal-guided attention (SURVEY 8e, exchange 2)."""
 
     def __init__(self, fwd_map: torch.Tensor, traj_mask: torch.Tensor, world: int, rank: int, chunks: int, group=None):
-        """fwd_map int64 [N, L] (trajectory p visits token fwd_map[f, p] of frame f); traj_mask uint8 [L, N, N]"""
+        """fwd_map int64 [N, L] (trajectory p visits token fwd_map[f, p] of frame f); traj_mask uint8 [L, N, N].  Rank s
+        owns frames ``frame_range(N, world, s)`` and trajectories ``frame_range(L, world, s)``; neither has to split
+        evenly."""
         N, L = fwd_map.shape
-        if L % world != 0:
-            raise ValueError(f"{L} trajectories do not split evenly over {world} ranks")
         self.world, self.rank, self.group, self.chunks = world, rank, group, chunks
-        self.N, self.L, self.Lg = N, L, L // world
+        self.N, self.L = N, L
         lo, hi = frame_range(N, world, rank)
         n_local = hi - lo
         self.n_local = n_local
+        traj = [frame_range(L, world, s) for s in range(world)]
+        t_lo, t_hi = traj[rank]
+        self.Lg = t_hi - t_lo
+        frames = block_sizes(N, world)
+        # all_to_all split sizes in rows, fixed for the batch: to rank s go my frames' rows of its trajectories; from
+        # rank r come r's frames' rows of mine
+        self.send_splits = [n_local * chunks * (b - a) for a, b in traj]
+        self.recv_splits = [f * chunks * self.Lg for f in frames]
         dev = fwd_map.device
-        # send row (s, j, b, t)  <-  local row (b * n_local + j) * L + fwd_map[lo + j, s * Lg + t]
-        fm = fwd_map[lo:hi].view(n_local, world, self.Lg).permute(1, 0, 2)                    # [s, j, t]
+        # send row (s, j, b, t)  <-  local row (b * n_local + j) * L + fwd_map[lo + j, traj[s][0] + t]
         brow = (torch.arange(chunks, device=dev)[None, :] * n_local + torch.arange(n_local, device=dev)[:, None]) * L   # [j, b]
-        idx = fm[:, :, None, :] + brow[None, :, :, None]                                     # [s, j, b, t]
-        self.row_idx = idx.reshape(-1).to(torch.int32).contiguous()
+        idx = [(fwd_map[lo:hi, a:b][:, None, :] + brow[:, :, None]).reshape(-1) for a, b in traj]   # [j, b, t] per s
+        self.row_idx = torch.cat(idx).to(torch.int32).contiguous()
         self.identity_map = torch.arange(chunks * self.Lg, device=dev, dtype=torch.int64)[None].expand(N, -1).contiguous()
-        mine = traj_mask[rank * self.Lg:(rank + 1) * self.Lg]                                 # [Lg, N, N]
+        mine = traj_mask[t_lo:t_hi]                                                           # [Lg, N, N]
         self.mask = mine[None].expand(chunks, -1, -1, -1).reshape(chunks * self.Lg, N, N).contiguous()
         self._bufs = {}
 
     def _buffers(self, C: int, like: torch.Tensor):
         key = (C, like.dtype)
         if key not in self._bufs:
-            n = self.world * self.n_local * self.chunks * self.Lg
-            mk = lambda w: torch.empty(n, w, dtype=like.dtype, device=like.device)
-            self._bufs[key] = (mk(3 * C), mk(3 * C), mk(C))
+            mk = lambda n, w: torch.empty(n, w, dtype=like.dtype, device=like.device)
+            local, mine = self.n_local * self.chunks * self.L, self.N * self.chunks * self.Lg
+            self._bufs[key] = (mk(local, 3 * C), mk(mine, 3 * C), mk(local, C))
         return self._bufs[key]
 
     def run(self, q, k, attn_out, heads: int, scale: float, backend) -> torch.Tensor:
@@ -198,11 +232,11 @@ class ShardedTrajectoryExchange:
         send, recv, back = self._buffers(C, q)
         for col, t in enumerate((q, k, attn_out)):
             backend.rows_gather(t.view(-1, C), self.row_idx, send, col * C)
-        dist.all_to_all_single(recv, send, group=self.group)
+        dist.all_to_all_single(recv, send, self.recv_splits, self.send_splits, group=self.group)
         # recv rows are ordered (source rank r, its frame j, chunk b, trajectory t) = (global frame, chunk * Lg + t)
         res = backend.temporal_attn_fwd_packed(recv.view(self.N, self.chunks * self.Lg, 3 * C), self.identity_map, self.mask,
                                                1, heads, scale)
-        dist.all_to_all_single(back, res.view(-1, C), group=self.group)
+        dist.all_to_all_single(back, res.view(-1, C), self.send_splits, self.recv_splits, group=self.group)
         out = torch.empty_like(attn_out)
         backend.rows_scatter(back, self.row_idx, out.view(-1, C))
         return out

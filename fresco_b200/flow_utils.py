@@ -112,7 +112,7 @@ def warp_tensor(sample, flows, occs, saliency, unet_chunk_size, shard=None):
     ranks (a decoded image has 3: background smoothing, src/pipe_FRESCO.py:46) every rank all-gathers the frames instead,
     runs the chain on the whole batch and keeps its own frames."""
     world = 1 if shard is None else shard[0]
-    n = sample.shape[0] // unet_chunk_size * world
+    n = sample.shape[0] // unet_chunk_size if world == 1 else flows[0].shape[0]
     h, w = sample.shape[2], sample.shape[3]
 
     def prepare():
@@ -146,26 +146,31 @@ def warp_tensor(sample, flows, occs, saliency, unet_chunk_size, shard=None):
     if world == 1:
         return chain(chain_input(sample.contiguous()), unet_chunk_size).to(sample.dtype)
     import torch.distributed as dist
-    from .dist import all_gather_blocks
+    from .dist import all_gather_frames, block_sizes, frame_range
     group = shard[2] if len(shard) > 2 else None
-    chunks, n_local, C = unet_chunk_size, n // world, sample.shape[1]
+    chunks, C = unet_chunk_size, sample.shape[1]
+    lo, hi = frame_range(n, world, shard[1])
+    n_local = hi - lo
+    if sample.shape[0] != chunks * n_local:
+        raise ValueError(f"warp_tensor: rank {shard[1]} of {world} owns frames [{lo}, {hi}) of {n}, "
+                         f"so sample needs {chunks * n_local} planes, got {sample.shape[0]}")
     if C % world != 0:
         # gather path: the frames travel in the dtype of ``sample`` (fp16 VAE output: 1.5 MB per 512^2 frame), the chain
         # runs on exactly the batch the unsharded call sees
-        full = all_gather_blocks(sample, world, group)                               # [rank, chunk, frame, C, h, w]
-        full = full.view(world, chunks, n_local, C, h, w).transpose(0, 1).reshape(chunks * n, C, h, w)
+        full = all_gather_frames(sample, n, world, chunks, group)                     # [chunk, frame, C, h, w]
         fused = chain(chain_input(full), chunks).view(chunks, n, C, h, w)
-        lo = shard[1] * n_local
-        return fused[:, lo:lo + n_local].reshape(chunks * n_local, C, h, w).to(sample.dtype)
+        return fused[:, lo:hi].reshape(chunks * n_local, C, h, w).to(sample.dtype)
     x = chain_input(sample.contiguous())
     cg = C // world
+    frames = block_sizes(n, world)                              # split sizes of the all-to-alls, in frames
     send = x.view(chunks, n_local, world, cg, h * w).permute(2, 1, 0, 3, 4).contiguous()      # [dest, frame, chunk, cg, hw]
-    recv = torch.empty_like(send)
-    dist.all_to_all_single(recv, send, group=group)            # [source rank = frame block, frame, chunk, cg, hw]
+    send = send.view(world * n_local, chunks * cg * h * w)
+    recv = torch.empty(n, chunks * cg * h * w, dtype=x.dtype, device=x.device)
+    dist.all_to_all_single(recv, send, frames, [n_local] * world, group=group)   # [source rank = frame block, frame, ...]
     planes = recv.view(n, chunks * cg, h, w)                    # all N frames x my channel slice of both chunks
     fused = chain(planes, 1)
-    back = torch.empty_like(fused)
-    dist.all_to_all_single(back, fused, group=group)           # [source rank = channel block, frame, chunk, cg, hw]
+    back = torch.empty_like(send)
+    dist.all_to_all_single(back, fused.view(n, -1), [n_local] * world, frames, group=group)   # [source = channel block, ...]
     out = back.view(world, n_local, chunks, cg, h * w).permute(2, 1, 0, 3, 4).reshape(chunks * n_local, C, h, w)
     return out.contiguous().to(sample.dtype)
 

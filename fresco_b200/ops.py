@@ -291,13 +291,19 @@ def gram_normalize(cs_bcl: torch.Tensor):
     return xhat, norms
 
 
+def _gram_scale(weight: float, B: int, Lt: int) -> float:
+    """loss scale of the Gram-L1 term, weight / (B * L^2), in double: the launcher rounds it to fp32 once, so a rank's
+    share of the weight (intra_weight * n / total) gives the same fp32 scale as the unsharded call"""
+    return float(weight) / (B * Lt * Lt)
+
+
 def gram_sign(xhat, target, weight: float, loss_acc=None):
     B, Lt, C = xhat.shape
     tsign = torch.empty(B, Lt, Lt, dtype=torch.float16, device=xhat.device)
     ev = _prof_begin()
-    L.check(L.lib().fresco_gram_sign(L.ptr(xhat), L.ptr(target), L.ptr(tsign),
-                                     L.ptr(loss_acc) if loss_acc is not None else None, B, Lt, C, float(weight),
-                                     L.stream()), "fresco_gram_sign")
+    L.check(L.lib().fresco_gram_sign_scaled(L.ptr(xhat), L.ptr(target), L.ptr(tsign),
+                                            L.ptr(loss_acc) if loss_acc is not None else None, B, Lt, C,
+                                            _gram_scale(weight, B, Lt), L.stream()), "fresco_gram_sign_scaled")
     _prof_end(ev, "gram_sign_C%d_L%d" % (C, Lt), 2.0 * B * Lt * Lt * C, "tensor")       # SURVEY 8d: forward Gram
     return tsign
 
@@ -308,9 +314,9 @@ def gram_sign_ref(xhat, yhat, weight: float, loss_acc=None):
     B, Lt, C = xhat.shape
     tsign = torch.empty(B, Lt, Lt, dtype=torch.float16, device=xhat.device)
     ev = _prof_begin()
-    L.check(L.lib().fresco_gram_sign_ref(L.ptr(xhat), L.ptr(yhat), L.ptr(tsign),
-                                         L.ptr(loss_acc) if loss_acc is not None else None, B, Lt, C, float(weight),
-                                         L.stream()), "fresco_gram_sign_ref")
+    L.check(L.lib().fresco_gram_sign_ref_scaled(L.ptr(xhat), L.ptr(yhat), L.ptr(tsign),
+                                                L.ptr(loss_acc) if loss_acc is not None else None, B, Lt, C,
+                                                _gram_scale(weight, B, Lt), L.stream()), "fresco_gram_sign_ref_scaled")
     _prof_end(ev, "gram_sign_C%d_L%d" % (C, Lt), 2.0 * B * Lt * Lt * C, "tensor")       # SURVEY 8d: forward Gram
     return tsign
 
@@ -320,8 +326,9 @@ def gram_grad(tsign, xhat, norms, grad_bcl, weight: float):
     nbytes = int(L.lib().fresco_gram_grad_workspace_bytes(B, Lt, C))
     ws = _workspace(("gram_grad", xhat.device), max(nbytes, 16), xhat.device)
     ev = _prof_begin()
-    L.check(L.lib().fresco_gram_grad(L.ptr(tsign), L.ptr(xhat), L.ptr(norms), L.ptr(grad_bcl), B, Lt, C,
-                                     float(weight), L.ptr(ws), nbytes, L.stream()), "fresco_gram_grad")
+    L.check(L.lib().fresco_gram_grad_scaled(L.ptr(tsign), L.ptr(xhat), L.ptr(norms), L.ptr(grad_bcl), B, Lt, C,
+                                            _gram_scale(weight, B, Lt), L.ptr(ws), nbytes, L.stream()),
+            "fresco_gram_grad_scaled")
     _prof_end(ev, "gram_grad_C%d_L%d" % (C, Lt), 4.0 * B * Lt * Lt * C, "tensor")       # SURVEY 8d: the two backward products
     return grad_bcl
 

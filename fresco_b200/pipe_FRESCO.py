@@ -6,7 +6,7 @@ Same names, arguments and behaviour.  What changes underneath:
   fused kernels of libfresco_b200.so instead of ~15 torch ops (fresco_cfg_pred_x0 / fresco_ddpm_prev);
 * background smoothing calls this package's warp_tensor (image-resolution chain, dilation kernel);
 * ``inference(..., shard=(world, rank, group))`` (not in the reference) runs ONE keyframe batch frame-sharded over the
-  GPUs of a box: every rank holds frames [rank*N/G, (rank+1)*N/G); the initial noise and the per-step noise are drawn
+  GPUs of a box: every rank holds frames frame_range(N, G, rank) = [rank*N//G, (rank+1)*N//G); the initial noise and the per-step noise are drawn
   for ALL N frames from identically seeded generators on every rank and sliced, so the sample paths are those of the
   unsharded run (``repeat_noise`` needs frame 0's noise everywhere, :67-68, :150-151); ``record_latents`` (frames 0
   and N-1, :175-179) is assembled with one tiny all-gather per step; restoring frames 0-1 in propagation mode touches
@@ -90,7 +90,7 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
     """Video-to-video translation of one keyframe batch with FRESCO (src/pipe_FRESCO.py:81-234).
 
     ``imgs`` / ``edges`` / ``prompt_embeds`` / ``flows`` / ``occs`` / ``saliency`` hold ALL N frames (every rank gets the
-    same arguments); with ``shard=(world, rank[, group])`` this rank denoises frames [rank*N/G, (rank+1)*N/G) and
+    same arguments); with ``shard=(world, rank[, group])`` this rank denoises frames [rank*N//G, (rank+1)*N//G) and
     returns their latents, the background-smoothing steps included."""
     device = pipe._execution_device
     noise_scheduler = pipe.scheduler

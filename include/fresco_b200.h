@@ -166,6 +166,16 @@ int fresco_gram_sign_ref(const void* xhat, const void* yhat, void* tsign, float*
                          int channels, float weight, void* stream);
 int fresco_gram_tx(const void* tsign, const void* xhat, float* ghat, int batch, int tokens, int channels, float alpha,
                    void* stream);
+/* the three steps above with the loss scale given directly: `scale` multiplies every |D| of the loss and the T xhat
+ * product of the gradient, and is rounded to fp32 once.  The `weight` forms pass (double)weight/(batch*tokens^2).  A
+ * frame-sharded caller passes the scale of the whole batch, intra_weight/(chunks*total_frames*tokens^2), computed in
+ * double: rounding a rank's share of the weight to fp32 first would give a scale that differs from the unsharded one. */
+int fresco_gram_sign_scaled(const void* xhat, const float* target, void* tsign, float* loss_acc, int batch, int tokens,
+                            int channels, double scale, void* stream);
+int fresco_gram_sign_ref_scaled(const void* xhat, const void* yhat, void* tsign, float* loss_acc, int batch, int tokens,
+                                int channels, double scale, void* stream);
+int fresco_gram_grad_scaled(const void* tsign, const void* xhat, const float* norms, float* grad, int batch, int tokens,
+                            int channels, double scale, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- O4 / O5: Adam update and AdaIN ---------------------------------------------------------
  * fresco_adam_step replaces torch.optim.Adam.step at src/diffusion_hacked.py:433,485
