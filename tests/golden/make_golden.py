@@ -1,6 +1,6 @@
 """Generate golden vectors by running the REAL reference (williamyang1991/FRESCO) on CPU.
 
-    python tests/golden/make_golden.py [--set b] --reference /path/to/FRESCO
+    python tests/golden/make_golden.py [--set b | --only gmflow_rect] --reference /path/to/FRESCO
 
 The reference imports two diffusers names and matplotlib at module top
 (src/diffusion_hacked.py:7-8, src/utils.py:5); neither is used on the path we
@@ -183,8 +183,37 @@ def scenario_b(dh, fu, geometry, matching, ut):
     print("golden fixture set B written to", HERE)
 
 
+def scenario_gmflow_rect(matching):
+    """``--only gmflow_rect``: GMFlow's global correlation (both directions and one) and the split-window attention
+    (with and without shift) on a NON-SQUARE 24 x 40 grid: L = 960 tokens, 7.5 key tiles of 128 (the last one ragged);
+    2 x 2 windows of 12 x 20 and shifted regions down to 6 x 10.  Inputs are fp16-representable, so the fp16 kernels
+    read exactly these operands."""
+    from gmflow import transformer as T
+    g = torch.Generator().manual_seed(960)
+    b, c, h, w = 2, 64, 24, 40
+    f0 = (torch.randn(b, c, h, w, generator=g) * 1.5).half().float()
+    f1 = (torch.roll(f0, shifts=(2, -3), dims=(2, 3)) + 0.5 * torch.randn(b, c, h, w, generator=g)).half().float()
+    res = {"f0": f0.half().numpy(), "f1": f1.half().numpy(),
+           "flow_bidir": matching.global_correlation_softmax(f0, f1, pred_bidir_flow=True)[0].numpy(),
+           "flow_uni": matching.global_correlation_softmax(f0, f1, pred_bidir_flow=False)[0].numpy()}
+    cw = 128
+    q = (torch.randn(1, h * w, cw, generator=g) * 1.5).half().float()
+    k = torch.randn(1, h * w, cw, generator=g).half().float()
+    v = torch.randn(1, h * w, cw, generator=g).half().float()
+    res.update(q=q.half().numpy(), k=k.half().numpy(), v=v.half().numpy(), h=h, w=w)
+    res["out_split"] = T.single_head_split_window_attention(q, k, v, num_splits=2, with_shift=False, h=h, w=w).numpy()
+    mask = T.generate_shift_window_attn_mask((h, w), h // 2, w // 2, h // 4, w // 4, device=torch.device("cpu"))
+    res["out_shift"] = T.single_head_split_window_attention(q, k, v, num_splits=2, with_shift=True, h=h, w=w,
+                                                            attn_mask=mask).numpy()
+    save_npz("gmflow_rect", **res)
+    print("gmflow_rect fixture written to", HERE)
+
+
 def main():
     dh, fu, geometry, matching, ut = import_reference()
+    torch.set_grad_enabled(False)
+    if "--only" in sys.argv and sys.argv[sys.argv.index("--only") + 1] == "gmflow_rect":
+        return scenario_gmflow_rect(matching)
     if "--set" in sys.argv and sys.argv[sys.argv.index("--set") + 1] == "b":
         return scenario_b(dh, fu, geometry, matching, ut)
     torch.manual_seed(0)

@@ -29,6 +29,7 @@ import torch.nn.functional as F
 
 from oracle import attention_bound as AB
 from oracle import fresco_oracle as O
+from oracle import gmflow_bound as GB
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "fresco_b200", "csrc")
@@ -419,7 +420,8 @@ row("chain-per-step-half-rejected", [], _chain_rejects_fp16_image_planes)
 
 # ================================================================================================ GMFlow flow attention
 def _gmflow_flow_attention(fb, launch, B=16, L=4096, C=128, seed=0):
-    """GMFlow's flow propagation at 512 x 512: 64 x 64 tokens, V a flow field of tens of pixels."""
+    """GMFlow's flow propagation at 512 x 512: 64 x 64 tokens, V a flow field of tens of pixels; elementwise within
+    oracle.gmflow_bound."""
     g = torch.Generator(device="cuda").manual_seed(seed)
     q = (torch.randn(B, L, C, device="cuda", generator=g) * 2.0).half()
     k = torch.randn(B, L, C, device="cuda", generator=g).half()
@@ -427,11 +429,9 @@ def _gmflow_flow_attention(fb, launch, B=16, L=4096, C=128, seed=0):
     out = _nan((B, 2, L), torch.float32)
     scale = 1.0 / math.sqrt(C)
     launch("gmflow_flow_attention", fb.c.gmflow_flow_attention(P(q), P(k), P(vals), P(out), B, L, C, scale, fb.lib.stream()))
-    bound = 1e-4 * vals.abs().max().item()
-    for b in range(B):
-        s = (q[b].double() @ k[b].double().T) * scale
-        ref = (torch.softmax(s, -1) @ vals[b].double()).T
-        _check_close(out[b], ref, bound, f"flow attention batch {b}")
+    ref, tol = GB.flow_attn_ref_and_bound(q, k, vals, scale)
+    ratio = (out.double() - ref).abs() / tol
+    assert not (ratio > 1).any() and torch.isfinite(out).all(), "flow attention: " + _worst_tile(ratio.flatten(0, 1))
 
 
 row("gmflow-flow-attention-16x4096x128", ["tile_gemm_kernel<EPI_GMFLOW,0>"], _gmflow_flow_attention)
@@ -565,7 +565,8 @@ COVERED_ELSEWHERE = {
     "ddpm_prev_kernel<half>": "test_gpu_parity_r2.py::test_ddpm_step_kernels_and_dilate_golden",
     "ddpm_prev_kernel<float>": "test_gpu_parity_r2.py::test_ddpm_step_kernels_and_dilate_golden",
     "dilate_kernel": "test_gpu_parity_r2.py::test_ddpm_step_kernels_and_dilate_golden",
-    "to_token_major_f16_kernel": "test_gpu_kernels.py::test_gmflow_global_correlation (first launches of the call)",
+    "to_token_major_f16_kernel": "test_gpu_gmflow.py::test_corr_families (the first two launches of every call; the "
+                                 "fp16 rounding it does is what gmflow_bound evaluates)",
     "mapping_single_kernel": "test_gpu_kernels.py::test_mapping_bit_exact_golden",
 }
 

@@ -108,6 +108,25 @@ def test_gmflow_global_correlation(golden):
     assert (fu - T(g["flow_uni"])).abs().max() < 1e-4
 
 
+def test_gmflow_global_correlation_rectangular_ragged(golden):
+    """24 x 40 grid (L = 960: 7.5 key tiles of 128), both directions and one: the oracle in fp32 and in fp64 against the
+    reference.  The fp64 distance is the fixture's own fp32 error, which tests/test_gpu_gmflow.py adds to the kernel's
+    bound when it checks the kernel against this fixture."""
+    g = golden("gmflow_rect")
+    f0, f1 = T(g["f0"]).float(), T(g["f1"]).float()
+    assert f0.shape == (2, 64, 24, 40)
+    for bidir, key in ((True, "flow_bidir"), (False, "flow_uni")):
+        ref = T(g[key])
+        assert ref.shape[0] == (4 if bidir else 2)
+        fo, _ = O.global_correlation_softmax(f0, f1, bidir)
+        assert (fo - ref).abs().max() < 1e-4, key
+        f64, _ = O.global_correlation_softmax(f0.double(), f1.double(), bidir)
+        assert (f64 - ref.double()).abs().max() < 1e-4, key
+    fb, _ = O.global_correlation_softmax(f0, f1, True)
+    fu, _ = O.global_correlation_softmax(f0, f1, False)
+    assert torch.equal(fb[:2], fu)                                   # [fwd(B), bwd(B)]: the forward half first
+
+
 def test_set_b_odd_frames_nonsquare_head_dim_80(golden):
     """Fixture set B (N = 3 frames, 64 x 96 plane, head_dim 80): mapping, attention, warp_tensor, optimize_feature."""
     g = golden("set_b")
