@@ -180,18 +180,38 @@ def _workspace(key, nbytes: int, device) -> torch.Tensor:
 
 
 def warp_adjoint_ell(flow: torch.Tensor):
-    """Per-batch operands of the temporal-consistency loss for the warp by ``flow`` [F,2,h,w]:
-    the ADJOINT of that warp in ELL form, row = destination pixel, up to 8 entries (round(w*65535) << 16) | source in
-    uint32, used slots first (``ell_packed`` [F, hw, 8]); destinations with more than 8 taps spill to ``ovf`` int32
-    [F, n_ovf, 3] = (destination | -1, source, float bits of the weight)."""
+    """Per-batch operands of the temporal-consistency loss for the warp by ``flow`` [F,2,h,w]: the bilinear taps of
+    every source pixel (fresco_warp_taps) packed into the ADJOINT of that warp by :func:`_pack_adjoint`."""
     Fr, _, h, w = flow.shape
-    hw = h * w
-    dev = flow.device
-    dest = torch.empty(Fr, hw, 4, dtype=torch.int32, device=dev)
-    wgt = torch.empty(Fr, hw, 4, dtype=torch.float32, device=dev)
+    dest = torch.empty(Fr, h * w, 4, dtype=torch.int32, device=flow.device)
+    wgt = torch.empty(Fr, h * w, 4, dtype=torch.float32, device=flow.device)
     L.check(L.lib().fresco_warp_taps(L.ptr(flow), L.ptr(dest), L.ptr(wgt), Fr, h, w, L.stream()), "fresco_warp_taps")
-    dest = dest.reshape(Fr, 4 * hw).long()
-    wgt = wgt.reshape(Fr, 4 * hw)
+    return _pack_adjoint(dest, wgt, h, w)
+
+
+def _pack_adjoint(dest: torch.Tensor, wgt: torch.Tensor, h: int, w: int):
+    """Taps dest int [F, hw, 4] (-1 = none) / wgt fp32 [F, hw, 4] of the warp -> its ADJOINT in ELL form, row =
+    destination pixel, up to 8 entries (round(w*65535) << 16) | source in uint32 (``ell_packed`` [F, hw, 8]);
+    destinations with more than 8 taps spill to ``ovf`` int32 [F, n_ovf, 3] = (destination | -1, source, float bits
+    of the weight).  Pure torch (runs on any device).
+
+    Invariant the loss kernels rely on: a row's used slots come first and a slot whose weight field is 0 ends the row
+    (warp_loss_quad_kernel stops a warp's walk at the first slot that is 0 in all of its lanes).  A tap whose weight
+    rounds to a 0 field (w < 2^-17) is therefore dropped, from the ELL and from the overflow list alike: it would
+    contribute nothing through the ELL anyway, and it sorts by source, so it can come before the row's main tap.
+    (The loss kernels also take keep masks in {0, 1}: their fp16 sgn(r) * keep planes are exact only for those.)"""
+    Fr = dest.shape[0]
+    dest = dest.reshape(Fr, -1)
+    wgt = wgt.reshape(Fr, -1)
+    return _pack_ell(torch.where((wgt * 65535.0).round() > 0, dest, torch.full_like(dest, -1)), wgt, h, w)
+
+
+def _pack_ell(dest: torch.Tensor, wgt: torch.Tensor, h: int, w: int):
+    """The packing of :func:`_pack_adjoint` for every tap with dest >= 0, whatever its weight (dest, wgt [F, 4 hw])."""
+    Fr = dest.shape[0]
+    hw = h * w
+    dev = dest.device
+    dest = dest.long()
     src = torch.arange(hw, device=dev).repeat_interleave(4)[None].expand(Fr, -1)
     key = torch.where(dest >= 0, dest, torch.full_like(dest, hw))            # tap-less entries sort to the end
     order = torch.argsort(key, dim=1, stable=True)

@@ -114,9 +114,13 @@ int fresco_warp_fuse_chain(const void* sample, void* out, int is_half, const flo
 /* ---- O2: temporal-consistency loss, forward + backward -------------------------------------
  * replaces src/diffusion_hacked.py:461-466 and its autograd backward.
  * cs, grad float [chunks, frames, channels, h, w]; fwd_flow/bwd_flow float [frames,2,h,w];
- * fwd_keep/bwd_keep float [frames,h,w] (= 1 - occlusion).  The adjoint of the bilinear warp is applied as a
- * gather through a per-frame ELL matrix built once per batch from fresco_warp_taps + a sort by destination:
- * *_ell uint32 [frames, h*w, 8], entry = (round(weight*65535) << 16) | source pixel (0 = empty slot);
+ * fwd_keep/bwd_keep float [frames,h,w] (= 1 - occlusion), each value 0 or 1 (what every caller passes: max_pool of
+ * binary occlusions); the quad and group kernels store sgn(r) * keep in fp16, exact only for such masks.  The adjoint
+ * of the bilinear warp is applied as a gather through a per-frame ELL matrix built once per batch from
+ * fresco_warp_taps + a sort by destination:
+ * *_ell uint32 [frames, h*w, 8], entry = (round(weight*65535) << 16) | source pixel (0 = empty slot).  A row's used
+ * slots come first and a slot whose weight field is 0 ends the row (the quad kernel stops a warp's walk there), so a
+ * tap whose weight rounds to a 0 field (< 2^-17) is left out of the ELL and the overflow list alike;
  * overflow int32 [2 (bwd,fwd), frames, n_overflow, 3] = (destination | -1, source, float bits of weight) for
  * destinations with more than 8 taps.  h*w <= 65535.  grad is overwritten (accumulate=0) or added to;
  * *loss_acc (device float, may be null) gets the loss value added.
