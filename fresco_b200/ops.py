@@ -92,11 +92,35 @@ def attn_fwd_kv_packed(q: torch.Tensor, kv: torch.Tensor, heads: int, q_per_kv: 
     return out
 
 
+def _check_temporal_operands(what, tensors, width, fwd_map, traj_mask, chunks, heads):
+    """Refuse, before any launch, operands the kernels would reinterpret: the C ABI takes raw pointers, so an fp32 q, an
+    int32 map or a mask of the wrong shape would otherwise be read as fp16 / int64 / [tokens, N, N] bytes."""
+    if any(t.dtype != torch.float16 or t.dim() != 3 for t in tensors):
+        raise L.FrescoError(f"{what}: q, k, v must be fp16 [chunks*frames, tokens, C]")
+    B, tokens, C = tensors[0].shape
+    if any(t.shape != tensors[0].shape for t in tensors) or C % width:
+        raise L.FrescoError(f"{what}: q, k, v shapes differ")
+    C //= width
+    if chunks <= 0 or B % chunks:
+        raise L.FrescoError(f"{what}: {B} rows do not split into {chunks} chunks")
+    if heads <= 0 or C % heads:
+        raise L.FrescoError(f"{what}: C = {C} is not a multiple of heads = {heads}")
+    frames = B // chunks
+    if fwd_map.dtype != torch.int64 or tuple(fwd_map.shape) != (frames, tokens):
+        raise L.FrescoError(f"{what}: fwd_map must be int64 [{frames}, {tokens}], got {fwd_map.dtype} "
+                            f"{list(fwd_map.shape)}")
+    if traj_mask.dtype not in (torch.uint8, torch.bool) or tuple(traj_mask.shape) != (tokens, frames, frames):
+        raise L.FrescoError(f"{what}: traj_mask must be uint8 or bool [{tokens}, {frames}, {frames}], got "
+                            f"{traj_mask.dtype} {list(traj_mask.shape)}")
+    return frames, tokens, C
+
+
 def temporal_attn_fwd_packed(qkv: torch.Tensor, fwd_map, traj_mask, chunks: int, heads: int, scale: float):
     """qkv [chunks*frames, tokens, 3C] with q | k | v side by side in every row -> out [chunks*frames, tokens, C]."""
-    B, tokens, C3 = qkv.shape
-    C = C3 // 3
-    frames = B // chunks
+    frames, tokens, C = _check_temporal_operands("temporal_attn_fwd_packed", (qkv,), 3, fwd_map, traj_mask, chunks,
+                                                 heads)
+    B = qkv.shape[0]
+    C3 = 3 * C
     out = torch.empty(B, tokens, C, dtype=qkv.dtype, device=qkv.device)
     base = L.ptr(qkv)
     ev = _prof_begin()
@@ -127,8 +151,11 @@ def attn_fwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, q_pe
 
 
 def temporal_attn_fwd(q_raw, k_raw, v_src, fwd_map, traj_mask, chunks: int, heads: int, scale: float):
-    B, tokens, C = q_raw.shape
-    frames = B // chunks
+    """q_raw, k_raw, v_src [chunks*frames, tokens, C] fp16; fwd_map int64 [frames, tokens]; traj_mask uint8 / bool
+    [tokens, frames, frames] -> out like v_src (include/fresco_b200.h, A5)."""
+    frames, tokens, C = _check_temporal_operands("temporal_attn_fwd", (q_raw, k_raw, v_src), 1, fwd_map, traj_mask,
+                                                 chunks, heads)
+    B = q_raw.shape[0]
     out = torch.empty_like(v_src)
     ev = _prof_begin()
     L.check(L.lib().fresco_temporal_attn_fwd(L.ptr(q_raw), L.ptr(k_raw), L.ptr(v_src), L.ptr(out), L.ptr(fwd_map),

@@ -82,8 +82,12 @@ int fresco_attn_fwd_kv_strided(const void* q, const void* k, const void* v, void
  * replaces src/diffusion_hacked.py:320-367.
  * q_raw, k_raw, v_src, out  half [chunks*frames, tokens, heads*head_dim]  (v_src = output of A4)
  * fwd_map int64 [frames, tokens] (trajectory p sits at token fwd_map[f][p] of frame f; a permutation)
- * traj_mask uint8 [tokens, frames, frames] (1 = attend)
- * out[b,f,fwd_map[f][p]] = sum_g softmax_g(q[f,pos]·k[g,pos] * scale, masked) v[g,pos]          */
+ * traj_mask uint8 [tokens, frames, frames] (traj_mask[p][f][g] = 1: frame f of trajectory p attends to frame g).
+ *   Every row traj_mask[p][f][.] must keep at least one key; the reference's masks always keep the diagonal, and
+ *   the kernels rely on a finite row maximum (a fully masked row is undefined input).
+ * out[b,f,fwd_map[f][p]] = sum_g softmax_g(q[f,pos]·k[g,pos] * scale, masked) v[g,pos]
+ * frames > 16 run only with dense inputs (in_row_stride == heads*head_dim): the strided entry point returns
+ * FRESCO_ERR_UNSUPPORTED there.                                                                 */
 int fresco_temporal_attn_fwd(const void* q_raw, const void* k_raw, const void* v_src, void* out,
                              const int64_t* fwd_map, const uint8_t* traj_mask, int chunks, int frames, int tokens,
                              int heads, int head_dim, float scale, void* stream);

@@ -10,7 +10,8 @@ the options, and the kernels the call must launch, in order, as ``fresco_last_ke
   fails here instead of quietly moving a row to another kernel,
 * compares the output with a plain fp64 reference of the same operation, evaluated on the operands the kernel consumes
   (fp16-rounded where the kernel reads fp16).  The temporal-consistency loss rows are held elementwise to
-  ``oracle.warp_loss_bound`` (``tests/test_gpu_warp_loss.py`` runs its input families on every loss kernel).
+  ``oracle.warp_loss_bound`` (``tests/test_gpu_warp_loss.py`` runs its input families on every loss kernel), the
+  temporal attention rows to ``oracle.temporal_bound`` (``tests/test_gpu_temporal_attention.py``).
 
 Instantiations no row reaches are listed with the reason in ``NOT_LAST`` (launched, but another kernel of the same
 call is what the record shows) or ``COVERED_ELSEWHERE`` (one instantiation per dtype, no selection; the named test
@@ -30,6 +31,7 @@ import torch.nn.functional as F
 from oracle import attention_bound as AB
 from oracle import fresco_oracle as O
 from oracle import gmflow_bound as GB
+from oracle import temporal_bound as TB
 from oracle import warp_loss_bound as WB
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -123,28 +125,12 @@ def _trajectories(N, L, seed):
     return fwd, mask
 
 
-def _temporal_ref(q, k, v, fwd, mask, chunks, heads, scale):
-    """fp64: out[b, f, fwd[f, p]] = softmax_g(q[f, .] . k[g, .] * scale, masked) v[g, .] along trajectory p."""
-    B, L, C = q.shape
-    N, d = B // chunks, C // heads
-    pos = fwd.cuda()
-    fr = torch.arange(N, device="cuda")[:, None]
-    m = mask.cuda()[:, None]
-    out = torch.empty(B, L, C, dtype=torch.float64, device="cuda")
-    for b in range(chunks):
-        sl = slice(b * N, (b + 1) * N)
-        qb, kb, vb = (t[sl][fr, pos].double().reshape(N, L, heads, d) for t in (q, k, v))
-        s = torch.einsum("flhd,glhd->lhfg", qb, kb) * scale
-        p = torch.softmax(s.masked_fill(~m, float("-inf")), -1)
-        ob = out[sl]
-        ob[fr, pos] = torch.einsum("lhfg,glhd->flhd", p, vb).reshape(N, L, C)
-    return out
-
-
-def _temporal(fb, launch, N, L, heads, d, packed=False, chunks=2, seed=0):
+def _temporal(fb, launch, N, L, heads, d, packed=False, chunks=2, seed=0, kernel="rows"):
     """packed=False: fresco_temporal_attn_fwd on dense [chunks*N, L, C] tensors.  packed=True: the call
     ShardedTrajectoryExchange.run makes -- qkv [N, chunks*L, 3C] with q | k | v in every row, identity map, chunks=1,
-    mask [chunks*L, N, N] (L = this rank's trajectories)."""
+    mask [chunks*L, N, N] (L = this rank's trajectories).  Every element within oracle.temporal_bound for ``kernel``
+    (rows: temporal_attn_rows_kernel, round1: temporal_attn_kernel); tests/test_gpu_temporal_attention.py runs the
+    bound's input families on both kernels."""
     C, scale = heads * d, 1.0 / math.sqrt(d)
     g = torch.Generator(device="cuda").manual_seed(seed)
     fwd, mask = _trajectories(N, L, seed)
@@ -170,13 +156,15 @@ def _temporal(fb, launch, N, L, heads, d, packed=False, chunks=2, seed=0):
     launch("fresco_temporal_attn_fwd_strided",
            fb.c.fresco_temporal_attn_fwd_strided(pq, pk, pv, P(out), P(fwd_d), P(mask_d), kchunks, N, tokens, heads, d,
                                                  stride, scale, fb.lib.stream()))
-    ref = _temporal_ref(q, k, v, fwd, mask, kchunks, heads, scale)
-    # the stated fp16 attention bound, over every output row
-    _check_close(out, ref, 2e-3 * ref.abs().max().item(), "temporal attention")
+    ref, tol = TB.ref_and_bound(q, k, v, fwd_d, mask_d, kchunks, heads, scale, kernel)
+    ratio = TB.ratio(out, ref, tol)
+    assert not (ratio > 1).any(), "temporal attention: " + _worst_tile(ratio.reshape(-1, C))
 
 
 for _N, _d, _L in [(9, 40, 4096), (12, 40, 4096), (16, 40, 4096), (9, 80, 1024), (12, 80, 1024), (16, 80, 1024)]:
-    # N = 16, 8 heads: 128 rows per trajectory, so 2 trajectories per CTA at d = 40 and 1 at d = 80 (48 KB)
+    # N = 16, 8 heads: 128 rows per trajectory, so at most 2 trajectories per CTA.  Each takes 2 * N * 2C bytes of
+    # shared memory (+ 4 N): 20 KB at d = 40, so 2 per CTA; 40 KB at d = 80, where 2 would exceed the 48 KB the
+    # launcher keeps a CTA under, so 1
     row(f"temporal-N{_N}-d{_d}", [f"temporal_attn_rows_kernel<{_d},16>"], _temporal, N=_N, L=_L, heads=8, d=_d)
 row("temporal-N8-d40", ["temporal_attn_rows_kernel<40,8>"], _temporal, N=8, L=4096, heads=8, d=40)
 row("temporal-N4-d80", ["temporal_attn_rows_kernel<80,8>"], _temporal, N=4, L=1024, heads=8, d=80)
@@ -187,11 +175,11 @@ row("temporal-packed-N16-d40", ["temporal_attn_rows_kernel<40,16>"], _temporal, 
 row("temporal-packed-N16-d80", ["temporal_attn_rows_kernel<80,16>"], _temporal, N=16, L=1024 // 2, heads=8, d=80,
     packed=True)
 row("temporal-packed-N5-d64", ["temporal_attn_rows_kernel<64,8>"], _temporal, N=5, L=300, heads=4, d=64, packed=True)
-row("temporal-round1-N17-d40", ["temporal_attn_kernel"], _temporal, N=17, L=1024, heads=8, d=40)
-row("temporal-round1-N24-d80", ["temporal_attn_kernel"], _temporal, N=24, L=512, heads=8, d=80)
-row("temporal-round1-N4-d128", ["temporal_attn_kernel"], _temporal, N=4, L=300, heads=2, d=128)
+row("temporal-round1-N17-d40", ["temporal_attn_kernel"], _temporal, N=17, L=1024, heads=8, d=40, kernel="round1")
+row("temporal-round1-N24-d80", ["temporal_attn_kernel"], _temporal, N=24, L=512, heads=8, d=80, kernel="round1")
+row("temporal-round1-N4-d128", ["temporal_attn_kernel"], _temporal, N=4, L=300, heads=2, d=128, kernel="round1")
 row("temporal-V1-N8-d40", ["temporal_attn_kernel"], _temporal, opts={"FRESCO_TEMPORAL_V": 1}, N=8, L=4096, heads=8,
-    d=40)
+    d=40, kernel="round1")
 
 
 # ================================================================================================ cross-frame attention
