@@ -58,6 +58,13 @@ _SIGNATURES = {
     "fresco_ddpm_prev": (c_int, [_P, _P, _P, _P, c_int, c_longlong, c_longlong, c_int, c_float, c_float, c_float, _P]),
     "fresco_mapping_single": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P, _P, _P, c_size_t, _P]),
     "fresco_mapping_workspace_bytes": (c_size_t, [c_int]),
+    "fresco_blend_lut_gather": (c_int, [_P, _P, _P, c_longlong, _P]),
+    "fresco_blend_mask_chain": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, _P]),
+    "fresco_blend_histogram": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, _P, c_size_t, _P]),
+    "fresco_blend_poisson": (c_int, [_P, _P, _P, _P, c_double, c_double, c_double, _P, _P, c_int, c_int, c_int, _P,
+                                     c_size_t, _P]),
+    "fresco_blend_cheby_iterations": (c_int, [c_int, c_int, c_double]),
+    "fresco_blend_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -24,8 +24,12 @@ FLAGS = [f for f in FLAGS if f != "--use_fast_math=false"]
 FLAGS += os.environ.get("FRESCO_NVCC_EXTRA", "").split()      # extra nvcc flags for experimental builds
 
 
+# the propagation stage's blending kernels (csrc/blend/) are a separate component from the keyframe path's (csrc/)
+BLEND = os.path.join(CSRC, "blend")
+
+
 def sources():
-    return sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cu"))
+    return sorted(os.path.join(d, f) for d in (CSRC, BLEND) for f in os.listdir(d) if f.endswith(".cu"))
 
 
 def _stale(target, deps):

@@ -467,3 +467,130 @@ def mapping_single(bwd_flow: torch.Tensor, bwd_occ: torch.Tensor, imgs: torch.Te
                                           L.ptr(mapping), L.ptr(unlinked), L.ptr(ws), nbytes, L.stream()),
             "fresco_mapping_single")
     return mapping, unlinked.bool()
+
+
+# ---- B1: propagation-stage frame blending (include/fresco_b200.h) ----
+
+def _check_blend(what, **named):
+    """Refuse, before any launch, operands the blend kernels would reinterpret: each entry is name -> (tensor, dtype,
+    shape), with None in the shape for a free dimension."""
+    for name, (t, dtype, shape) in named.items():
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise L.FrescoError(f"{what}: {name} must be a CUDA tensor")
+        if t.dtype != dtype:
+            raise L.FrescoError(f"{what}: {name} must be {dtype}, got {t.dtype}")
+        if t.dim() != len(shape) or any(s is not None and s != d for s, d in zip(shape, t.shape)):
+            raise L.FrescoError(f"{what}: {name} must have shape {list(shape)}, got {list(t.shape)}")
+        if not t.is_contiguous():
+            raise L.FrescoError(f"{what}: {name} must be contiguous")
+
+
+def blend_lut_gather(img: torch.Tensor, lut: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """uint8 [..., 3] colour triples -> lut[triple] (lut uint8 [2^24, 3], cv2's conversion of every triple)."""
+    if img.dim() < 1:
+        raise L.FrescoError("blend_lut_gather: img must be uint8 [..., 3]")
+    _check_blend("blend_lut_gather", img=(img, torch.uint8, (None,) * (img.dim() - 1) + (3,)),
+                 lut=(lut, torch.uint8, (1 << 24, 3)))
+    if out is None:
+        out = torch.empty_like(img)
+    _check_blend("blend_lut_gather", out=(out, torch.uint8, tuple(img.shape)))
+    n = img.numel() // 3
+    if n:
+        ev = _prof_begin()
+        L.check(L.lib().fresco_blend_lut_gather(L.ptr(img), L.ptr(lut), L.ptr(out), n, L.stream()),
+                "fresco_blend_lut_gather")
+        _prof_end(ev, "blend_lut_gather", 9.0 * n, "hbm")      # 3 bytes in, 3 gathered, 3 out per pixel
+    return out
+
+
+def blend_mask_chain(dist1: torch.Tensor, dist2: torch.Tensor, flows: torch.Tensor,
+                     out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Error masks of one sequence, each OR'd with the previous one warped by its backward flow.  dist1, dist2 fp32
+    [interval-1, h, w]; flows fp32 [interval-1, 2, h, w] (flow 0 unused) -> uint8 [interval-1, h, w] in {0, 1}."""
+    if dist1.dim() != 3:
+        raise L.FrescoError("blend_mask_chain: dist1 must be fp32 [interval-1, h, w]")
+    F_, h, w = dist1.shape
+    _check_blend("blend_mask_chain", dist1=(dist1, torch.float32, (F_, h, w)), dist2=(dist2, torch.float32, (F_, h, w)),
+                 flows=(flows, torch.float32, (F_, 2, h, w)))
+    if out is None:
+        out = torch.empty(F_, h, w, dtype=torch.uint8, device=dist1.device)
+    _check_blend("blend_mask_chain", out=(out, torch.uint8, (F_, h, w)))
+    ev = _prof_begin()
+    L.check(L.lib().fresco_blend_mask_chain(L.ptr(dist1), L.ptr(dist2), L.ptr(flows), L.ptr(out), F_ + 1, h, w,
+                                            L.stream()), "fresco_blend_mask_chain")
+    _prof_end(ev, "blend_mask_chain_%dx%d" % (h, w), 17.0 * F_ * h * w, "hbm")    # 2 dists, flow, mask in, mask out
+    return out
+
+
+def _blend_workspace(frames: int, h: int, w: int, device) -> torch.Tensor:
+    nbytes = int(L.lib().fresco_blend_workspace_bytes(frames, h, w))
+    return _workspace(("blend", device), nbytes, device)
+
+
+def blend_histogram(lab_a: torch.Tensor, lab_b: torch.Tensor, weights: torch.Tensor,
+                    lab_min_error: Optional[torch.Tensor] = None, masks: Optional[torch.Tensor] = None,
+                    out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """blender/histogram_blend.blend in Lab, before its Lab -> BGR: lab_a, lab_b uint8 [F, h, w, 3]; weights fp64
+    [F, 2] (blend's weight1, weight2); the min-error image either given (uint8 [F, h, w, 3]) or selected from a (mask 0)
+    and b (mask 1) by masks uint8 [F, h, w]."""
+    if lab_a.dim() != 4:
+        raise L.FrescoError("blend_histogram: lab_a must be uint8 [frames, h, w, 3]")
+    F_, h, w, _ = lab_a.shape
+    img = (F_, h, w, 3)
+    args = dict(lab_a=(lab_a, torch.uint8, img), lab_b=(lab_b, torch.uint8, img),
+                weights=(weights, torch.float64, (F_, 2)))
+    if (lab_min_error is None) == (masks is None):
+        raise L.FrescoError("blend_histogram: pass exactly one of lab_min_error and masks")
+    if lab_min_error is not None:
+        args["lab_min_error"] = (lab_min_error, torch.uint8, img)
+    else:
+        args["masks"] = (masks, torch.uint8, (F_, h, w))
+    _check_blend("blend_histogram", **args)
+    if out is None:
+        out = torch.empty_like(lab_a)
+    _check_blend("blend_histogram", out=(out, torch.uint8, img))
+    ws = _blend_workspace(F_, h, w, lab_a.device)
+    ev = _prof_begin()
+    L.check(L.lib().fresco_blend_histogram(
+        L.ptr(lab_a), L.ptr(lab_b), L.ptr(lab_min_error) if lab_min_error is not None else None,
+        L.ptr(masks) if masks is not None else None, L.ptr(weights), L.ptr(out), F_, h, w, L.ptr(ws), ws.numel(),
+        L.stream()), "fresco_blend_histogram")
+    _prof_end(ev, "blend_histogram_%dx%d" % (h, w), 34.0 * F_ * h * w, "hbm")    # 4 passes over a, b, mask + the output
+    return out
+
+
+def blend_cheby_iterations(h: int, w: int, weight: float) -> int:
+    """Chebyshev steps fresco_blend_poisson runs for one channel (oracle/blend_bound.py derives the count)."""
+    return int(L.lib().fresco_blend_cheby_iterations(int(h), int(w), float(weight)))
+
+
+def blend_poisson(lab_target: torch.Tensor, lab_a: torch.Tensor, lab_b: torch.Tensor, masks: torch.Tensor,
+                  grad_weight=(2.5, 0.5, 0.5), out: Optional[torch.Tensor] = None,
+                  solution: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """blender/poisson_fusion.poisson_fusion in Lab, before its Lab -> BGR: the exact least-squares solution per
+    channel, clipped to [0, 255] and truncated.  Images uint8 [F, h, w, 3], masks uint8 [F, h, w]; ``solution`` fp64
+    [F, 3, h, w], if given, receives the unclipped solution."""
+    if lab_target.dim() != 4:
+        raise L.FrescoError("blend_poisson: lab_target must be uint8 [frames, h, w, 3]")
+    F_, h, w, _ = lab_target.shape
+    img = (F_, h, w, 3)
+    _check_blend("blend_poisson", lab_target=(lab_target, torch.uint8, img), lab_a=(lab_a, torch.uint8, img),
+                 lab_b=(lab_b, torch.uint8, img), masks=(masks, torch.uint8, (F_, h, w)))
+    gw = [float(x) for x in grad_weight]
+    if len(gw) != 3:
+        raise L.FrescoError("blend_poisson: grad_weight must have one weight per channel")
+    if out is None:
+        out = torch.empty_like(lab_target)
+    _check_blend("blend_poisson", out=(out, torch.uint8, img))
+    if solution is not None:
+        _check_blend("blend_poisson", solution=(solution, torch.float64, (F_, 3, h, w)))
+    ws = _blend_workspace(F_, h, w, lab_target.device)
+    ev = _prof_begin()
+    L.check(L.lib().fresco_blend_poisson(L.ptr(lab_target), L.ptr(lab_a), L.ptr(lab_b), L.ptr(masks), gw[0], gw[1],
+                                         gw[2], L.ptr(out), L.ptr(solution) if solution is not None else None, F_, h,
+                                         w, L.ptr(ws), ws.numel(), L.stream()), "fresco_blend_poisson")
+    if ev is not None:
+        # every Chebyshev step reads the iterate (5-point, cached), the previous iterate and b, and writes one plane
+        iters = sum(blend_cheby_iterations(h, w, x) for x in gw)
+        _prof_end(ev, "blend_poisson_%dx%d" % (h, w), 32.0 * F_ * h * w * iters, "hbm")
+    return out

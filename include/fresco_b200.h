@@ -234,6 +234,32 @@ int fresco_mapping_single(const float* bwd_flow, const float* bwd_occ, const flo
                           void* stream);
 size_t fresco_mapping_workspace_bytes(int tokens);
 
+/* ---- B1: propagation-stage frame blending ---------------------------------------------------
+ * replaces video_blend.py:172-255 with blender/histogram_blend.py:19-50 and blender/poisson_fusion.py:54-93.
+ * Images are uint8 [frames, h, w, 3] (BGR or cv2 8-bit Lab), masks uint8 [frames, h, w] in {0, 1}.
+ * lut_gather: out[p] = lut[(in[p][0] << 16 | in[p][1] << 8 | in[p][2])], lut uint8 [2^24, 3] (cv2's conversion of
+ *   every triple, built by the caller).
+ * mask_chain: frame k = 0 .. interval-2 of one sequence: error mask of dist1/dist2 float [interval-1, h, w] with
+ *   weight1 = k / (interval-1), OR'd with frame k-1's mask warped (nearest, torch CPU grid_sample bit for bit) by
+ *   flows float [interval-1, 2, h, w] (flow 0 unused; may be null when interval == 2).
+ * histogram: blend() in Lab; lab_min_error may be null, then the min-error image is a where mask is 0, b where 1;
+ *   weights double [frames, 2] are blend()'s weight1, weight2 per frame.
+ * poisson: the exact least-squares solution of poisson_fusion's system per Lab channel (Chebyshev iteration in fp64,
+ *   fresco_blend_cheby_iterations(h, w, weight) steps), clip [0, 255], truncated; `solution` double
+ *   [frames, 3, h, w] (may be null) receives the unclipped solution.
+ * workspace: fresco_blend_workspace_bytes(frames, h, w) (histogram and poisson).                              */
+int fresco_blend_lut_gather(const uint8_t* in, const uint8_t* lut, uint8_t* out, long long pixels, void* stream);
+int fresco_blend_mask_chain(const float* dist1, const float* dist2, const float* flows, uint8_t* masks, int interval,
+                            int h, int w, void* stream);
+int fresco_blend_histogram(const uint8_t* lab_a, const uint8_t* lab_b, const uint8_t* lab_min_error,
+                           const uint8_t* masks, const double* weights, uint8_t* lab_out, int frames, int h, int w,
+                           void* workspace, size_t workspace_bytes, void* stream);
+int fresco_blend_poisson(const uint8_t* lab_target, const uint8_t* lab_a, const uint8_t* lab_b, const uint8_t* masks,
+                         double weight0, double weight1, double weight2, uint8_t* lab_out, double* solution,
+                         int frames, int h, int w, void* workspace, size_t workspace_bytes, void* stream);
+int fresco_blend_cheby_iterations(int h, int w, double weight);
+size_t fresco_blend_workspace_bytes(int frames, int h, int w);
+
 #ifdef __cplusplus
 }
 #endif
