@@ -204,6 +204,32 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
+// One warp fills a [128 rows x 64 fp16] K-major atom of src[row, k] (row stride ld elements) in the layout a
+// SWIZZLE_128B TMA box gives it (16-byte chunk c of row r at r * 128 + ((c ^ (r & 7)) << 4)), zero outside
+// rows < n_rows, k < n_k.  For an operand whose row stride is not a multiple of 16 bytes, which no tensor map can
+// describe: its rows may be only 2-byte aligned, so the loads are per element.  The caller fences the generic-proxy
+// stores (fence_proxy_async_smem) before it signals the atom to wgmma.
+__device__ __forceinline__ void fill_kmajor_atom_sw128(uint8_t* dst, const __half* src, size_t ld, int row0, int k0,
+                                                       int n_rows, int n_k, int lane) {
+  const unsigned short* s = reinterpret_cast<const unsigned short*>(src);
+#pragma unroll 4
+  for (int t = lane; t < 128 * 8; t += 32) {
+    const int r = t >> 3, c = t & 7;
+    const int gr = row0 + r, gk = k0 + c * 8;
+    uint32_t w[4];
+#pragma unroll
+    for (int e = 0; e < 8; e += 2) {
+      const size_t off = (size_t)gr * ld + gk + e;
+      const uint32_t lo = (gr < n_rows && gk + e < n_k) ? __ldg(s + off) : 0u;
+      const uint32_t hi = (gr < n_rows && gk + e + 1 < n_k) ? __ldg(s + off + 1) : 0u;
+      w[e >> 1] = lo | (hi << 16);
+    }
+    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(smem_u32(dst + r * 128 + ((c ^ (r & 7)) << 4))),
+                 "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3])
+                 : "memory");
+  }
+}
+
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

@@ -8,6 +8,10 @@
 // 64-element swizzle atoms through a 3-stage TMA/mbarrier ring (producer: warp 8) and accumulated by wgmma in the
 // registers of two consumer warpgroups (64 rows each), which then run the epilogue on their own accumulators while the
 // producer already streams the next column tile.
+//
+// RAGGED (EPI_STORE with an MN-major B, i.e. fresco_gram_grad's T Xh at tokens % 8 != 0): A = T [batch, M, M] fp16
+// has a row stride of 2M bytes, which no tensor map can describe; the whole producer warp fills its atoms in the
+// swizzled layout TMA would give them, B keeps its tensor map.  The consumers are the same code.
 #include "common.cuh"
 #include "fresco_internal.h"
 
@@ -39,11 +43,12 @@ struct GemmParams {
   float scale_log2;
   const float2* vals;         // optional V [batch, N] (2 channels per key); null: V = the key's (x, y) pixel coordinate and
                               // the query's own coordinate is subtracted from the result (flow = correspondence - grid)
+  const __half* a_ptr;        // RAGGED: A [batch, M, K], read without a tensor map
 };
 
 __device__ __forceinline__ float sign3(float d) { return d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f); }
 
-template <int EPI, bool B_MN>
+template <int EPI, bool B_MN, bool RAGGED = false>
 __global__ void __launch_bounds__(kGThreads, 1)
 tile_gemm_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                  const GemmParams p) {
@@ -59,10 +64,11 @@ tile_gemm_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
   const int batch = blockIdx.z;
   const int n_tile0 = blockIdx.x * p.n_iter;
   const int k_atoms = (p.K + 63) / 64;
+  static_assert(!RAGGED || (EPI == EPI_STORE && B_MN), "the ragged A operand is T of fresco_gram_grad");
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kGStages; ++s) {
-      mbar_init(bar_full + s, 1);
+      mbar_init(bar_full + s, RAGGED ? 32 : 1);          // RAGGED: every lane of the producer warp arrives
       mbar_init(bar_empty + s, 8);
     }
     fence_barrier_init();
@@ -70,6 +76,29 @@ tile_gemm_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
   __syncthreads();
 
   if (warp == 8) {
+    if constexpr (RAGGED) {
+      // ---------------------------------------------------------------- producer: A by the warp, B by TMA
+      int it = 0;
+      for (int t = 0; t < p.n_iter; ++t) {
+        const int n0 = (n_tile0 + t) * 128;
+        for (int ka = 0; ka < k_atoms; ++ka, ++it) {
+          const int st = it % kGStages;
+          if (it >= kGStages) mbar_wait_mma_backoff(bar_empty + st, ((it / kGStages) - 1) & 1, 64);
+          uint8_t* sa = smem + st * kGStageBytes;
+          uint8_t* sb = sa + kGAtomA;
+          fill_kmajor_atom_sw128(sa, p.a_ptr + (size_t)batch * p.M * p.K, p.K, m0, ka * 64, p.M, p.K, lane);
+          fence_proxy_async_smem();                       // the generic stores, before wgmma reads them
+          if (lane == 0) {
+            mbar_expect_tx(bar_full + st, kGStageBytes - kGAtomA);
+            tma_load_3d(sb, &tm_b, bar_full + st, n0, ka * 64, batch);
+            tma_load_3d(sb + 8192, &tm_b, bar_full + st, n0 + 64, ka * 64, batch);
+          } else {
+            mbar_arrive(bar_full + st);
+          }
+        }
+      }
+      return;
+    }
     // ------------------------------------------------------------------ TMA producer
     if (FRESCO_ISSUER_THREAD(lane)) {
       tma_prefetch_desc(&tm_a);
@@ -219,6 +248,13 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmP
   return check_launchf("tile_gemm_kernel<%s,%d>", kEpiNames[EPI], (int)B_MN);
 }
 
+static int launch_gemm_ragged_a(const CUtensorMap& tb, const GemmParams& p, dim3 grid, cudaStream_t s) {
+  const void* k = (const void*)tile_gemm_kernel<EPI_STORE, true, true>;
+  if (int rc = allow_dynamic_smem(k, kGSmem, "tile_gemm")) return rc;
+  tile_gemm_kernel<EPI_STORE, true, true><<<grid, kGThreads, kGSmem, s>>>(tb, tb, p);
+  return check_launch("tile_gemm_kernel<EPI_STORE,1,ragged>");
+}
+
 // ghat [batch, L, C] fp32 (token-major)  ->  grad [batch, C, L] += (ghat - (ghat . xhat) xhat) / norm
 // one CTA per (batch, 32 tokens); the row dot needs the whole C extent, hence the separate pass
 __global__ void gram_project_kernel(const float* __restrict__ ghat, const __half* __restrict__ xhat,
@@ -290,8 +326,9 @@ using namespace fresco;
 extern "C" int fresco_gram_sign_scaled(const void* xhat, const float* target, void* tsign, float* loss_acc, int batch,
                                        int tokens, int channels, double scale, void* stream) {
   if (!xhat || !target || !tsign) return set_error(FRESCO_ERR_ARG, "fresco_gram_sign: null pointer");
-  if (batch <= 0 || tokens <= 0 || channels <= 0 || channels % 8 != 0 || tokens % 8 != 0)
-    return set_error(FRESCO_ERR_ARG, "fresco_gram_sign: tokens and channels must be multiples of 8");
+  // the target and T are read and written element by element in the epilogue, so any token count runs here
+  if (batch <= 0 || tokens <= 0 || channels <= 0 || channels % 8 != 0)
+    return set_error(FRESCO_ERR_ARG, "fresco_gram_sign: channels must be a multiple of 8");
   CUtensorMap ta;
   if (make_kmajor_map(&ta, xhat, tokens, channels, batch, 128)) return FRESCO_ERR_TENSORMAP;
   GemmParams p = {};
@@ -321,8 +358,8 @@ extern "C" int fresco_gram_grad_scaled(const void* tsign, const void* xhat, cons
                                        int tokens, int channels, double scale, void* workspace, size_t workspace_bytes,
                                        void* stream) {
   if (!tsign || !xhat || !norms || !grad || !workspace) return set_error(FRESCO_ERR_ARG, "fresco_gram_grad: null pointer");
-  if (batch <= 0 || tokens <= 0 || channels <= 0 || channels % 8 != 0 || tokens % 8 != 0)
-    return set_error(FRESCO_ERR_ARG, "fresco_gram_grad: tokens and channels must be multiples of 8");
+  if (batch <= 0 || tokens <= 0 || channels <= 0 || channels % 8 != 0)
+    return set_error(FRESCO_ERR_ARG, "fresco_gram_grad: channels must be a multiple of 8");
   if (workspace_bytes < fresco_gram_grad_workspace_bytes(batch, tokens, channels))
     return set_error(FRESCO_ERR_ARG, "fresco_gram_grad: workspace too small");
   cudaStream_t s = (cudaStream_t)stream;
@@ -332,8 +369,9 @@ extern "C" int fresco_gram_grad_scaled(const void* tsign, const void* xhat, cons
     // persistent 128 x 256 tiles (gram_wgmma.cu)
     rc = fresco_gram_tx(tsign, xhat, static_cast<float*>(workspace), batch, tokens, channels, alpha, stream);
   } else {
+    const bool ragged = tokens % 8 != 0;            // T's rows are not 16-byte aligned: no tensor map for it
     CUtensorMap ta, tb;
-    if (make_kmajor_map(&ta, tsign, tokens, tokens, batch, 128)) return FRESCO_ERR_TENSORMAP;
+    if (!ragged && make_kmajor_map(&ta, tsign, tokens, tokens, batch, 128)) return FRESCO_ERR_TENSORMAP;
     if (make_mnmajor_map(&tb, xhat, tokens, channels, batch)) return FRESCO_ERR_TENSORMAP;
     GemmParams p = {};
     p.M = tokens;
@@ -342,7 +380,13 @@ extern "C" int fresco_gram_grad_scaled(const void* tsign, const void* xhat, cons
     p.n_iter = 1;
     p.out = static_cast<float*>(workspace);
     p.alpha = alpha;
-    rc = launch_gemm<EPI_STORE, true>(ta, tb, p, dim3((channels + 127) / 128, (tokens + 127) / 128, batch), s);
+    const dim3 grid((channels + 127) / 128, (tokens + 127) / 128, batch);
+    if (ragged) {
+      p.a_ptr = static_cast<const __half*>(tsign);
+      rc = launch_gemm_ragged_a(tb, p, grid, s);
+    } else {
+      rc = launch_gemm<EPI_STORE, true>(ta, tb, p, grid, s);
+    }
   }
   if (rc) return rc;
   const int tiles = (tokens + 31) / 32;

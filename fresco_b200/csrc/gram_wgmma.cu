@@ -9,6 +9,12 @@
 //              3, read every Adam iteration) is never materialised: what is stored per batch is Yh, [2N, L, C] fp16.
 //              Only tiles that touch the upper triangle are computed (D is symmetric).
 //   MODE_GRAD  Ghat = alpha * T Xh   (A = T, K-major; B = Xh read MN-major from its token-major layout), fp32 out.
+//
+// RAGGED (tokens % 8 != 0): T [batch, M, M] fp16 has a row stride of 2M bytes, which is not a multiple of 16, so no
+// tensor map can describe it.  MODE_SIGN then stores T element by element (a pair store would straddle rows and lose
+// its 4-byte alignment when M is odd); MODE_GRAD fills the A atom of every stage from the whole producer warp, in the
+// swizzled layout TMA would give it, while B (Xh, row stride 2C bytes) keeps its tensor map.  The wgmma consumers are
+// the same code.
 #include "common.cuh"
 #include "fresco_internal.h"
 
@@ -40,6 +46,7 @@ struct Gram2Params {
   // G2_GRAD
   float* out;                 // [batch, M, C]
   float alpha;
+  const __half* ta;           // G2_GRAD, RAGGED: T [batch, M, M], read without a tensor map
 };
 
 // tile id -> (batch, row tile I, column pair Jp) for G2_SIGN: row tile I needs the pairs that touch columns >= 128 I,
@@ -63,7 +70,7 @@ __device__ __forceinline__ void decode_tile(const Gram2Params& p, int tile, int&
   Jp = (I >> 1) + r;
 }
 
-template <int MODE>
+template <int MODE, bool RAGGED>
 __global__ void __launch_bounds__(kG2Threads, 1)
 gram2_kernel(const __grid_constant__ CUtensorMap tm_a0, const __grid_constant__ CUtensorMap tm_b0,
              const __grid_constant__ CUtensorMap tm_a1, const __grid_constant__ CUtensorMap tm_b1, const Gram2Params p) {
@@ -77,10 +84,11 @@ gram2_kernel(const __grid_constant__ CUtensorMap tm_a0, const __grid_constant__ 
   // K atoms (64 elements) of one tile: SIGN walks the channels twice (current features, then reference features)
   const int c_atoms = (p.C + 63) / 64;
   const int k_atoms = MODE == G2_SIGN ? 2 * c_atoms : (p.M + 63) / 64;
+  constexpr bool kWarpFill = RAGGED && MODE == G2_GRAD;    // the producer warp's 32 lanes each arrive on bar_full
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kG2Stages; ++s) {
-      mbar_init(bar_full + s, 1);
+      mbar_init(bar_full + s, kWarpFill ? 32 : 1);
       mbar_init(bar_empty + s, 8);
     }
     fence_barrier_init();
@@ -88,6 +96,31 @@ gram2_kernel(const __grid_constant__ CUtensorMap tm_a0, const __grid_constant__ 
   __syncthreads();
 
   if (warp == 8) {
+    if constexpr (kWarpFill) {
+      // ---------------------------------------------------------------- producer: A (T) by the warp, B (Xh) by TMA
+      int it = 0;
+      for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+        int b, I, Jp;
+        decode_tile<MODE>(p, tile, b, I, Jp);
+        for (int ka = 0; ka < k_atoms; ++ka, ++it) {
+          const int st = it % kG2Stages;
+          if (it >= kG2Stages) mbar_wait_mma_backoff(bar_empty + st, ((it / kG2Stages) - 1) & 1, 32);
+          uint8_t* sa = smem + st * kG2StageBytes;
+          uint8_t* sb = sa + kG2AtomA;
+          fill_kmajor_atom_sw128(sa, p.ta + (size_t)b * p.M * p.M, p.M, I * 128, ka * 64, p.M, p.M, lane);
+          fence_proxy_async_smem();                       // the generic stores, before wgmma reads them
+          if (lane == 0) {
+            mbar_expect_tx(bar_full + st, kG2AtomB);
+#pragma unroll
+            for (int q = 0; q < 4; ++q)
+              tma_load_3d(sb + q * 8192, &tm_b0, bar_full + st, Jp * 256 + q * 64, ka * 64, b);
+          } else {
+            mbar_arrive(bar_full + st);
+          }
+        }
+      }
+      return;
+    }
     // ------------------------------------------------------------------ TMA producer
     if (FRESCO_ISSUER_THREAD(lane)) {
       tma_prefetch_desc(&tm_a0);
@@ -184,10 +217,20 @@ gram2_kernel(const __grid_constant__ CUtensorMap tm_a0, const __grid_constant__ 
         loss += (fabsf(d0) + fabsf(d1)) * (diag ? 1.f : 2.f);   // off-diagonal blocks stand for their mirror as well
         const float t0 = d0 > 0.f ? 2.f : (d0 < 0.f ? -2.f : 0.f);
         const float t1 = d1 > 0.f ? 2.f : (d1 < 0.f ? -2.f : 0.f);
-        *reinterpret_cast<uint32_t*>(p.tsign + plane + (size_t)gm * p.M + j) = pack_half2(t0, t1);   // M % 8 == 0
-        if (!diag) {                                            // mirror T[j, i] = T[i, j]
-          p.tsign[plane + (size_t)j * p.M + gm] = __float2half_rn(t0);
-          p.tsign[plane + (size_t)(j + 1) * p.M + gm] = __float2half_rn(t1);
+        if constexpr (RAGGED) {                                 // j + 1 may be M; (gm, j) may be odd
+          const bool pair = j + 1 < p.M;
+          p.tsign[plane + (size_t)gm * p.M + j] = __float2half_rn(t0);
+          if (pair) p.tsign[plane + (size_t)gm * p.M + j + 1] = __float2half_rn(t1);
+          if (!diag) {
+            p.tsign[plane + (size_t)j * p.M + gm] = __float2half_rn(t0);
+            if (pair) p.tsign[plane + (size_t)(j + 1) * p.M + gm] = __float2half_rn(t1);
+          }
+        } else {
+          *reinterpret_cast<uint32_t*>(p.tsign + plane + (size_t)gm * p.M + j) = pack_half2(t0, t1);   // M % 8 == 0
+          if (!diag) {                                          // mirror T[j, i] = T[i, j]
+            p.tsign[plane + (size_t)j * p.M + gm] = __float2half_rn(t0);
+            p.tsign[plane + (size_t)(j + 1) * p.M + gm] = __float2half_rn(t1);
+          }
         }
       }
     }
@@ -198,13 +241,14 @@ gram2_kernel(const __grid_constant__ CUtensorMap tm_a0, const __grid_constant__ 
   }
 }
 
-template <int MODE>
+template <int MODE, bool RAGGED>
 static int launch_gram2(const CUtensorMap& a0, const CUtensorMap& b0, const CUtensorMap& a1, const CUtensorMap& b1,
                         const Gram2Params& p, cudaStream_t s) {
-  if (int rc = allow_dynamic_smem((const void*)gram2_kernel<MODE>, kG2Smem, "gram2")) return rc;
+  if (int rc = allow_dynamic_smem((const void*)gram2_kernel<MODE, RAGGED>, kG2Smem, "gram2")) return rc;
   int grid = sm_count();
   if (grid > p.n_tiles) grid = p.n_tiles;
-  gram2_kernel<MODE><<<grid, kG2Threads, kG2Smem, s>>>(a0, b0, a1, b1, p);
+  gram2_kernel<MODE, RAGGED><<<grid, kG2Threads, kG2Smem, s>>>(a0, b0, a1, b1, p);
+  if (RAGGED) return check_launch(MODE == G2_SIGN ? "gram2_kernel<G2_SIGN,ragged>" : "gram2_kernel<G2_GRAD,ragged>");
   return check_launch(MODE == G2_SIGN ? "gram2_kernel<G2_SIGN>" : "gram2_kernel<G2_GRAD>");
 }
 
@@ -215,8 +259,8 @@ using namespace fresco;
 extern "C" int fresco_gram_sign_ref_scaled(const void* xhat, const void* yhat, void* tsign, float* loss_acc, int batch,
                                            int tokens, int channels, double scale, void* stream) {
   if (!xhat || !yhat || !tsign) return set_error(FRESCO_ERR_ARG, "fresco_gram_sign_ref: null pointer");
-  if (batch <= 0 || tokens <= 0 || channels <= 0 || channels % 8 != 0 || tokens % 8 != 0)
-    return set_error(FRESCO_ERR_ARG, "fresco_gram_sign_ref: tokens and channels must be multiples of 8");
+  if (batch <= 0 || tokens <= 0 || channels <= 0 || channels % 8 != 0)
+    return set_error(FRESCO_ERR_ARG, "fresco_gram_sign_ref: channels must be a multiple of 8");
   CUtensorMap ax, bx, ay, by;
   if (make_kmajor_map(&ax, xhat, tokens, channels, batch, 128)) return FRESCO_ERR_TENSORMAP;
   if (make_kmajor_map(&bx, xhat, tokens, channels, batch, 256)) return FRESCO_ERR_TENSORMAP;
@@ -235,7 +279,8 @@ extern "C" int fresco_gram_sign_ref_scaled(const void* xhat, const void* yhat, v
   p.tsign = static_cast<__half*>(tsign);
   p.loss_acc = loss_acc;
   p.loss_scale = (float)scale;
-  return launch_gram2<G2_SIGN>(ax, bx, ay, by, p, (cudaStream_t)stream);
+  if (tokens % 8 != 0) return launch_gram2<G2_SIGN, true>(ax, bx, ay, by, p, (cudaStream_t)stream);
+  return launch_gram2<G2_SIGN, false>(ax, bx, ay, by, p, (cudaStream_t)stream);
 }
 
 extern "C" int fresco_gram_sign_ref(const void* xhat, const void* yhat, void* tsign, float* loss_acc, int batch,
@@ -247,11 +292,13 @@ extern "C" int fresco_gram_sign_ref(const void* xhat, const void* yhat, void* ts
 extern "C" int fresco_gram_tx(const void* tsign, const void* xhat, float* ghat, int batch, int tokens, int channels,
                               float alpha, void* stream) {
   if (!tsign || !xhat || !ghat) return set_error(FRESCO_ERR_ARG, "fresco_gram_tx: null pointer");
-  if (batch <= 0 || tokens <= 0 || channels <= 0 || channels % 8 != 0 || tokens % 8 != 0)
-    return set_error(FRESCO_ERR_ARG, "fresco_gram_tx: tokens and channels must be multiples of 8");
+  if (batch <= 0 || tokens <= 0 || channels <= 0 || channels % 8 != 0)
+    return set_error(FRESCO_ERR_ARG, "fresco_gram_tx: channels must be a multiple of 8");
+  const bool ragged = tokens % 8 != 0;              // T's rows are not 16-byte aligned: no tensor map for it
   CUtensorMap ta, tb;
-  if (make_kmajor_map(&ta, tsign, tokens, tokens, batch, 128)) return FRESCO_ERR_TENSORMAP;
+  if (!ragged && make_kmajor_map(&ta, tsign, tokens, tokens, batch, 128)) return FRESCO_ERR_TENSORMAP;
   if (make_mnmajor_map(&tb, xhat, tokens, channels, batch)) return FRESCO_ERR_TENSORMAP;
+  if (ragged) ta = tb;                              // unused by the ragged kernel
   Gram2Params p = {};
   p.M = tokens;
   p.C = channels;
@@ -262,5 +309,7 @@ extern "C" int fresco_gram_tx(const void* tsign, const void* xhat, float* ghat, 
   p.n_tiles = p.tiles_per_batch * batch;
   p.out = ghat;
   p.alpha = alpha;
-  return launch_gram2<G2_GRAD>(ta, tb, ta, tb, p, (cudaStream_t)stream);
+  p.ta = static_cast<const __half*>(tsign);
+  if (ragged) return launch_gram2<G2_GRAD, true>(ta, tb, ta, tb, p, (cudaStream_t)stream);
+  return launch_gram2<G2_GRAD, false>(ta, tb, ta, tb, p, (cudaStream_t)stream);
 }

@@ -157,7 +157,8 @@ int fresco_warp_loss_fwd_bwd_halo(const float* cs, const float* fwd_flow, const 
  *         written as half [batch, tokens, tokens]; loss += weight/(batch*tokens^2) * sum|G - A|.
  *         target float [batch, tokens, tokens] is the reference's correlation_matrix entry.
  * step 3  fresco_gram_grad (wgmma): ghat = T xhat * weight/(batch*tokens^2), projected through the
- *         normalisation Jacobian and added to grad float [batch, channels, tokens].             */
+ *         normalisation Jacobian and added to grad float [batch, channels, tokens].
+ * Every step takes any tokens >= 1 (channels a multiple of 8); T stays a contiguous half [batch, tokens, tokens].  */
 int fresco_gram_normalize(const float* cs, void* xhat, float* norms, int batch, int channels, int tokens,
                           void* stream);
 int fresco_gram_sign(const void* xhat, const float* target, void* tsign, float* loss_acc, int batch, int tokens,
