@@ -236,6 +236,9 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
+// sign of r as -1, 0 or +1 (0 for a zero residual), the derivative L1 losses use
+__device__ __forceinline__ float sgnf(float r) { return r > 0.f ? 1.f : (r < 0.f ? -1.f : 0.f); }
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

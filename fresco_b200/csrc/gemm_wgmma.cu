@@ -46,8 +46,6 @@ struct GemmParams {
   const __half* a_ptr;        // RAGGED: A [batch, M, K], read without a tensor map
 };
 
-__device__ __forceinline__ float sign3(float d) { return d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f); }
-
 template <int EPI, bool B_MN, bool RAGGED = false>
 __global__ void __launch_bounds__(kGThreads, 1)
 tile_gemm_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
@@ -177,7 +175,7 @@ tile_gemm_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
           const float d1 = acc[i] - __ldg(p.target + plane + (size_t)gm * p.M + gn);
           const float d2 = acc[i] - __ldg(p.target + plane + (size_t)gn * p.M + gm);
           loss += fabsf(d1) + (diag_tile ? 0.f : fabsf(d2));
-          const __half tv = __float2half_rn(sign3(d1) + sign3(d2));
+          const __half tv = __float2half_rn(sgnf(d1) + sgnf(d2));
           p.tsign[plane + (size_t)gm * p.M + gn] = tv;
           if (!diag_tile) p.tsign[plane + (size_t)gn * p.M + gm] = tv;
         }

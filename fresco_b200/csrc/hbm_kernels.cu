@@ -353,6 +353,98 @@ __device__ __forceinline__ float sample_taps(const PlaneT* plane, const Taps& t)
   return t.w00 * plane[t.i00] + t.w01 * plane[t.i01] + t.w10 * plane[t.i10] + t.w11 * plane[t.i11];
 }
 
+// four channels interleaved per pixel (the quad kernels' shared-memory planes)
+struct __align__(8) half4 {
+  __half2 lo, hi;
+};
+__device__ __forceinline__ float4 h4_to_f4(const half4& h) {
+  const float2 a = __half22float2(h.lo), b = __half22float2(h.hi);
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+__device__ __forceinline__ float4 sample_taps4(const float4* plane, const Taps& t) {
+  const float4 a0 = plane[t.i00], a1 = plane[t.i01], a2 = plane[t.i10], a3 = plane[t.i11];
+  return make_float4(t.w00 * a0.x + t.w01 * a1.x + t.w10 * a2.x + t.w11 * a3.x,
+                     t.w00 * a0.y + t.w01 * a1.y + t.w10 * a2.y + t.w11 * a3.y,
+                     t.w00 * a0.z + t.w01 * a1.z + t.w10 * a2.z + t.w11 * a3.z,
+                     t.w00 * a0.w + t.w01 * a1.w + t.w10 * a2.w + t.w11 * a3.w);
+}
+// fmaf(w, v, acc) for one channel or four
+__device__ __forceinline__ float fma_acc(float w, float v, float acc) { return fmaf(w, v, acc); }
+__device__ __forceinline__ float4 fma_acc(float w, const float4& v, const float4& acc) {
+  return make_float4(fmaf(w, v.x, acc.x), fmaf(w, v.y, acc.y), fmaf(w, v.z, acc.z), fmaf(w, v.w, acc.w));
+}
+
+// W1: one blend of the frame chain, z * (1 - m) + warp * m  (flow_utils.py:41-51); every chain kernel blends through
+// these, so they agree element for element
+__device__ __forceinline__ float chain_blend(float z, float warped, float m) { return z * (1.f - m) + warped * m; }
+__device__ __forceinline__ float4 chain_blend(const float4& z, const float4& warped, float m) {
+  return make_float4(chain_blend(z.x, warped.x, m), chain_blend(z.y, warped.y, m), chain_blend(z.z, warped.z, m),
+                     chain_blend(z.w, warped.w, m));
+}
+
+// ---- O2 (temporal-consistency loss): the steps the three loss kernels share.  The frame-sharded optimize_feature is
+//      bit-identical to the unsharded call only because every loss kernel sums in the fixed order written here.
+
+// One row of a warp adjoint in ELL form, as ops._pack_adjoint / ops._pack_ell build it: 8 uint32 slots per destination
+// pixel (two uint4), each (weight as unorm16) << 16 | (source pixel as u16).  A row's used slots come first, and a
+// slot whose weight field is 0 ends the row; unused slots are all-zero (weight 0, source 0), so reading one adds 0.
+struct EllRow {
+  uint32_t e[8];
+};
+__device__ __forceinline__ EllRow ell_load_row(const uint4* __restrict__ ell, int q) {
+  const uint4 e0 = __ldg(ell + 2 * q), e1 = __ldg(ell + 2 * q + 1);
+  return {{e0.x, e0.y, e0.z, e0.w, e1.x, e1.y, e1.z, e1.w}};
+}
+__device__ __forceinline__ bool ell_used(uint32_t slot) { return (slot >> 16) != 0; }
+__device__ __forceinline__ float ell_weight(uint32_t slot) { return (float)(slot >> 16) * (1.0f / 65535.0f); }
+__device__ __forceinline__ int ell_source(uint32_t slot) { return slot & 0xffffu; }
+
+// Overflow list of a warp adjoint: [n_ovf][3] int32 (destination, source, float bits of the weight) for the taps past
+// the 8 ELL slots of their destination, sorted by destination; -1 pads the tail.  The thread that holds the head of a
+// run sums the whole run in list order, with no atomics, so the result does not depend on scheduling.
+// value(source) is the sign plane at a source pixel: a float, or a float4 for a channel quad.
+__device__ __forceinline__ bool ovf_run_head(const int32_t* __restrict__ o, int e) {
+  return o[3 * e] >= 0 && (e == 0 || o[3 * (e - 1)] != o[3 * e]);
+}
+template <typename Value>
+__device__ __forceinline__ auto ovf_run_sum(const int32_t* __restrict__ o, int n_ovf, int e, Value value) {
+  decltype(value(0)) acc{};
+  for (int e2 = e; e2 < n_ovf && o[3 * e2] == o[3 * e]; ++e2)
+    acc = fma_acc(-__int_as_float(o[3 * e2 + 2]), value(o[3 * e2 + 1]), acc);
+  return acc;
+}
+
+// Frame f of the walk is paired with frame f + 1; after the last frame comes frame 0 (closed ring) or, in the open chain
+// of a frame-sharded batch, index `frames`, which the kernels' loaders read as the halo plane.
+__device__ __forceinline__ int next_frame(int f, int frames, bool open_chain) {
+  return (f + 1 == frames) ? (open_chain ? frames : 0) : f + 1;
+}
+
+// The gradient of frame f is its term ga of pair f plus the carry, what it received as the "next" frame of pair f - 1,
+// as two rounded products and one add: fl(fl(ga k) + fl(carry k)), never fl((ga + carry) k).  Frame 0 of the closed
+// ring receives carry_term() of the last pair in a second pass (add_carry); the open chain writes carry_term() to
+// halo_grad, and optimize_feature adds it to the next shard's first frame (`grad[:, 0] += from_prev`), which is the
+// same add, so the sharded gradient has the unsharded bits.
+__device__ __forceinline__ float carry_term(float carry, float k) { return __fmul_rn(carry, k); }
+__device__ __forceinline__ float add_carry(float g, float carry, float k) { return __fadd_rn(g, carry_term(carry, k)); }
+__device__ __forceinline__ float grad_term(float ga, float carry, float k) {
+  return __fadd_rn(__fmul_rn(ga, k), carry_term(carry, k));
+}
+
+// *loss_acc += k * (sum of every thread's loss in the CTA): warp sums, then one float atomic per CTA.  Every thread of
+// the CTA calls it.
+__device__ __forceinline__ void cta_loss_add(float loss, float* loss_acc, float k) {
+  __shared__ float red[32];
+  loss = warp_sum(loss);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = loss;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    float v = threadIdx.x < ((blockDim.x + 31) >> 5) ? red[threadIdx.x] : 0.f;
+    v = warp_sum(v);
+    if (threadIdx.x == 0) atomicAdd(loss_acc, v * k);
+  }
+}
+
 __global__ void flow_warp_kernel(const float* __restrict__ src, const float* __restrict__ flow,
                                  float* __restrict__ dst, int batch, int channels, int h, int w, int flow_batch) {
   const int hw = h * w;
@@ -434,7 +526,7 @@ warp_chain_group_kernel(const T* __restrict__ sample, T* __restrict__ out, const
       for (int kk = 0; kk < K; ++kk) z[kk] = live[kk] ? ld_as_float(sample + base[kk] + foff + i) : 0.f;
 #pragma unroll
       for (int kk = 0; kk < K; ++kk) {
-        const float v = z[kk] * (1.f - m) + sample_taps(cur + kk * hw, tp) * m;
+        const float v = chain_blend(z[kk], sample_taps(cur + kk * hw, tp), m);
         nxt[kk * hw + i] = v;
         if (!last && live[kk]) st_from_float(out + base[kk] + foff + i, v);
       }
@@ -458,32 +550,17 @@ warp_chain_group_kernel(const T* __restrict__ sample, T* __restrict__ out, const
     const float m = mk[i];
 #pragma unroll
     for (int kk = 0; kk < K; ++kk) {
-      const float v = cur[kk * hw + i] * (1.f - m) + sample_taps(nxt + kk * hw, tp) * m;
+      const float c = cur[kk * hw + i];
+      const float v = chain_blend(c, sample_taps(nxt + kk * hw, tp), m);
       if (live[kk]) st_from_float(out + base[kk] + loff + i, v);
     }
   }
 }
 
-struct __align__(8) half4 {
-  __half2 lo, hi;
-};
-__device__ __forceinline__ float4 h4_to_f4(const half4& h) {
-  const float2 a = __half22float2(h.lo), b = __half22float2(h.hi);
-  return make_float4(a.x, a.y, b.x, b.y);
-}
-__device__ __forceinline__ float sgnf(float r) { return r > 0.f ? 1.f : (r < 0.f ? -1.f : 0.f); }
-__device__ __forceinline__ float4 sample_taps4(const float4* plane, const Taps& t) {
-  const float4 a0 = plane[t.i00], a1 = plane[t.i01], a2 = plane[t.i10], a3 = plane[t.i11];
-  return make_float4(t.w00 * a0.x + t.w01 * a1.x + t.w10 * a2.x + t.w11 * a3.x,
-                     t.w00 * a0.y + t.w01 * a1.y + t.w10 * a2.y + t.w11 * a3.y,
-                     t.w00 * a0.z + t.w01 * a1.z + t.w10 * a2.z + t.w11 * a3.z,
-                     t.w00 * a0.w + t.w01 * a1.w + t.w10 * a2.w + t.w11 * a3.w);
-}
-
 // Channel-QUAD variant (the one warp_tensor runs on decoder features; see warp_loss_quad_kernel below for the
 // measurement behind it): NQ quads of four (chunk, channel) planes per CTA, interleaved per pixel as float4 in shared
 // memory, so the flows / blend weight of a pixel are fetched and its taps built once for 4 NQ channels and one 16-byte
-// shared load serves a tap for four of them.  Same arithmetic per element as warp_chain_group_kernel.
+// shared load serves a tap for four of them.  Same arithmetic per element as warp_chain_group_kernel (chain_blend).
 template <typename T, int P, int NQ>
 __global__ void __launch_bounds__(1024, 1)
 warp_chain_quad_kernel(const T* __restrict__ sample, T* __restrict__ out, const float* __restrict__ bwd_flow,
@@ -533,9 +610,7 @@ warp_chain_quad_kernel(const T* __restrict__ sample, T* __restrict__ out, const 
 #pragma unroll
       for (int nq = 0; nq < NQ; ++nq) {
         const float4 z = ld4(sample + base + foff + (long long)nq * 4 * hw, q);
-        const float4 wv = sample_taps4(cur + nq * hw, tp);
-        const float4 v = make_float4(z.x * (1.f - m) + wv.x * m, z.y * (1.f - m) + wv.y * m, z.z * (1.f - m) + wv.z * m,
-                                     z.w * (1.f - m) + wv.w * m);
+        const float4 v = chain_blend(z, sample_taps4(cur + nq * hw, tp), m);
         nxt[nq * hw + q] = v;
         if (!last) st4(out + base + foff + (long long)nq * 4 * hw, q, v);
       }
@@ -567,10 +642,7 @@ warp_chain_quad_kernel(const T* __restrict__ sample, T* __restrict__ out, const 
 #pragma unroll
       for (int nq = 0; nq < NQ; ++nq) {
         const float4 c = cur[nq * hw + q];
-        const float4 wv = sample_taps4(nxt + nq * hw, tp);
-        st4(out + base + loff + (long long)nq * 4 * hw, q,
-            make_float4(c.x * (1.f - m) + wv.x * m, c.y * (1.f - m) + wv.y * m, c.z * (1.f - m) + wv.z * m,
-                        c.w * (1.f - m) + wv.w * m));
+        st4(out + base + loff + (long long)nq * 4 * hw, q, chain_blend(c, sample_taps4(nxt + nq * hw, tp), m));
       }
     }
   }
@@ -592,7 +664,8 @@ __global__ void warp_blend_step_kernel(const float* __restrict__ src_frames, flo
     const float m = mask[i];
     const float* s = src_frames + ((long long)(j * frames + src_f) * channels + c) * hw;
     float* d = dst_frames + ((long long)(j * frames + dst_f) * channels + c) * hw;
-    d[i] = d[i] * (1.f - m) + sample_taps(s, tp) * m;
+    const float warped = sample_taps(s, tp);
+    d[i] = chain_blend(d[i], warped, m);
   }
 }
 
@@ -601,9 +674,9 @@ __global__ void warp_blend_step_kernel(const float* __restrict__ src_frames, flo
 // one CTA per (chunk, channel); frame pairs are walked sequentially with both planes in shared memory.
 // The backward of the bilinear warp (the adjoint W^T, a scatter-add in autograd) is evaluated as a GATHER:
 // W^T is the same sparse matrix for all chunks*channels planes of a frame pair, so it is built once per batch
-// (warp_taps_kernel + a sort on the host) in ELL form -- 8 packed (source:u16, weight:unorm16) slots per
-// destination pixel, 32 bytes per row -- and every plane just reads it: no atomics and no data-dependent loop
-// in the per-iteration kernel.  Destinations hit by more than 8 taps go to a small overflow list.
+// (warp_taps_kernel + a sort on the host) in ELL form (ell_load_row), and every plane just reads it: no atomics and
+// no data-dependent loop in the per-iteration kernel.  Destinations hit by more than 8 taps go to a small overflow
+// list (ovf_run_sum).
 // =============================================================================================
 __global__ void warp_taps_kernel(const float* __restrict__ flow, int32_t* __restrict__ dest,
                                  float* __restrict__ weight, int frames, int h, int w) {
@@ -623,11 +696,6 @@ __global__ void warp_taps_kernel(const float* __restrict__ flow, int32_t* __rest
       weight[t * 4 + k] = wt[k];
     }
   }
-}
-
-// overflow lists (destinations with more than 8 taps) are sorted by destination; -1 pads the tail
-__device__ __forceinline__ bool ovf_run_head(const int32_t* __restrict__ o, int e) {
-  return o[3 * e] >= 0 && (e == 0 || o[3 * (e - 1)] != o[3 * e]);
 }
 
 __global__ void warp_loss_kernel(const float* __restrict__ cs, const float* __restrict__ fwd_flow,
@@ -682,30 +750,29 @@ __global__ void warp_loss_kernel(const float* __restrict__ cs, const float* __re
         const float r = c2[i] - sample_taps(c1, tp);
         const float m = mb[i];
         loss += fabsf(r) * m;
-        s1[i] = (r > 0.f ? 1.f : (r < 0.f ? -1.f : 0.f)) * m * k;
+        s1[i] = sgnf(r) * m * k;
       }
       {  // r2 = c1 - W_ff(c2)
         const Taps tp = make_taps(x + ff[i], y + ff[hw + i], h, w);
         const float r = c1[i] - sample_taps(c2, tp);
         const float m = mf[i];
         loss += fabsf(r) * m;
-        s2[i] = (r > 0.f ? 1.f : (r < 0.f ? -1.f : 0.f)) * m * k;
+        s2[i] = sgnf(r) * m * k;
       }
     }
     __syncthreads();
     const bool a_add = accumulate || f > 0;                     // frame f   : first touched at f == 0
     const bool b_add = !to_halo && (accumulate || f == frames - 1);   // frame f+1 : first touched here, except the wrap to 0
-    // adjoint as a gather: 8 packed (source, weight) slots per destination pixel (ELL), two 16-byte loads per row
+    // adjoint as a gather through the ELL rows: all 8 slots of a row, unconditionally (an unused slot adds 0)
     const uint4* eb = bwd_ell + (long long)f * hw * 2;
     const uint4* ef = fwd_ell + (long long)f * hw * 2;
     float* ga = grad + plane_of(f);
     float* gb = to_halo ? halo_grad + halo_off : grad + plane_of(fn);
     auto gather8 = [&](const uint4* ell, int q, const float* sv) {
-      const uint4 e0 = __ldg(ell + 2 * q), e1 = __ldg(ell + 2 * q + 1);
-      const uint32_t e[8] = {e0.x, e0.y, e0.z, e0.w, e1.x, e1.y, e1.z, e1.w};
+      const EllRow r = ell_load_row(ell, q);
       float acc = 0.f;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) acc = fmaf((float)(e[j] >> 16) * (1.0f / 65535.0f), sv[e[j] & 0xffffu], acc);
+      for (int j = 0; j < 8; ++j) acc = fmaf(ell_weight(r.e[j]), sv[ell_source(r.e[j])], acc);
       return acc;
     };
     // d/dc1 = s2 - W_bf^T s1      (frame f)
@@ -725,38 +792,14 @@ __global__ void warp_loss_kernel(const float* __restrict__ cs, const float* __re
       __syncthreads();
       const int32_t* ob = ovf + ((long long)0 * frames + f) * n_ovf * 3;
       const int32_t* of = ovf + ((long long)1 * frames + f) * n_ovf * 3;
-      // entries are sorted by destination: the thread that holds the head of a run sums the run in list order (no
-      // atomics: the result does not depend on scheduling, which the frame-sharded bit-identity tests rely on)
-      for (int e = threadIdx.x; e < n_ovf; e += blockDim.x) {
-        if (ovf_run_head(ob, e)) {
-          float acc = 0.f;
-          for (int e2 = e; e2 < n_ovf && ob[3 * e2] == ob[3 * e]; ++e2)
-            acc = fmaf(-__int_as_float(ob[3 * e2 + 2]), s1[ob[3 * e2 + 1]], acc);
-          ga[ob[3 * e]] += acc;
-        }
-      }
+      for (int e = threadIdx.x; e < n_ovf; e += blockDim.x)
+        if (ovf_run_head(ob, e)) ga[ob[3 * e]] += ovf_run_sum(ob, n_ovf, e, [&](int src) { return s1[src]; });
       __syncthreads();                                          // (frames <= 2: ga and gb may be the same plane)
-      for (int e = threadIdx.x; e < n_ovf; e += blockDim.x) {
-        if (ovf_run_head(of, e)) {
-          float acc = 0.f;
-          for (int e2 = e; e2 < n_ovf && of[3 * e2] == of[3 * e]; ++e2)
-            acc = fmaf(-__int_as_float(of[3 * e2 + 2]), s2[of[3 * e2 + 1]], acc);
-          gb[of[3 * e]] += acc;
-        }
-      }
+      for (int e = threadIdx.x; e < n_ovf; e += blockDim.x)
+        if (ovf_run_head(of, e)) gb[of[3 * e]] += ovf_run_sum(of, n_ovf, e, [&](int src) { return s2[src]; });
     }
   }
-  if (loss_acc != nullptr) {
-    __shared__ float red[32];
-    loss = warp_sum(loss);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = loss;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      float v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
-      v = warp_sum(v);
-      if (threadIdx.x == 0) atomicAdd(loss_acc, v * k);
-    }
-  }
+  if (loss_acc != nullptr) cta_loss_add(loss, loss_acc, k);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -826,7 +869,7 @@ warp_loss_group_kernel(const float* __restrict__ cs, const float* __restrict__ f
 
   load_plane(cur, 0);
   for (int f = 0; f < frames; ++f) {
-    const int fn = (f + 1 == frames) ? (halo_cs != nullptr ? frames : 0) : f + 1;
+    const int fn = next_frame(f, frames, halo_cs != nullptr);
     load_plane(nxt, fn);
     __syncthreads();
     // ---- residuals of pair (f, fn): taps once per pixel, applied to the KT planes of this thread
@@ -851,32 +894,26 @@ warp_loss_group_kernel(const float* __restrict__ cs, const float* __restrict__ f
           const float r1 = c2[q] - sample_taps(c1, tb);       // c2 - W_bf(c1)
           const float r2 = c1[q] - sample_taps(c2, tf);       // c1 - W_ff(c2)
           loss += fabsf(r1) * mb + fabsf(r2) * mf;
-          s1[slot * hw + q] = __float2half_rn((r1 > 0.f ? 1.f : (r1 < 0.f ? -1.f : 0.f)) * mb);
-          s2[slot * hw + q] = __float2half_rn((r2 > 0.f ? 1.f : (r2 < 0.f ? -1.f : 0.f)) * mf);
+          s1[slot * hw + q] = __float2half_rn(sgnf(r1) * mb);
+          s2[slot * hw + q] = __float2half_rn(sgnf(r2) * mf);
         }
       }
     }
     __syncthreads();
     // ---- destinations hit by more than 8 taps of the backward-flow warp: their extra terms of d/dc1 (frame f) go
-    //      through the dead frame-f planes and join ga BEFORE it meets the carry -- a frame-sharded batch adds the carry
-    //      of a shard's first frame on the host and must see the same association.  Entries are sorted by destination:
-    //      the thread that holds the head of a run sums the run in list order (no atomics, deterministic).
+    //      through the dead frame-f planes and join ga BEFORE it meets the carry (grad_term)
     if (n_ovf > 0) {
       for (int idx = t; idx < K * hw; idx += T) cur[idx] = 0.f;
       __syncthreads();
       const int32_t* ob = ovf + ((long long)0 * frames + f) * n_ovf * 3;
       for (int e = t; e < n_ovf; e += T) {
         if (!ovf_run_head(ob, e)) continue;
-        for (int slot = 0; slot < K; ++slot) {
-          float acc = 0.f;
-          for (int e2 = e; e2 < n_ovf && ob[3 * e2] == ob[3 * e]; ++e2)
-            acc = fmaf(-__int_as_float(ob[3 * e2 + 2]), __half2float(s1[slot * hw + ob[3 * e2 + 1]]), acc);
-          cur[slot * hw + ob[3 * e]] = acc;
-        }
+        for (int slot = 0; slot < K; ++slot)
+          cur[slot * hw + ob[3 * e]] = ovf_run_sum(ob, n_ovf, e, [&](int src) { return __half2float(s1[slot * hw + src]); });
       }
       __syncthreads();
     }
-    // ---- adjoints as gathers (8 packed (source, weight) ELL slots per destination pixel), decoded once per pixel
+    // ---- adjoints as gathers through the ELL rows, each decoded once per pixel for the KT planes; unused slots skipped
     const uint4* ebp = bwd_ell + (long long)f * hw * 2;
     const uint4* efp = fwd_ell + (long long)f * hw * 2;
     const long long goff_a = (long long)f * fstride;
@@ -892,40 +929,29 @@ warp_loss_group_kernel(const float* __restrict__ cs, const float* __restrict__ f
         gb[kk] = __half2float(s1[slot * hw + q]);             // d/dc2 = s1 - W_ff^T s2   (frame fn)
         if (n_ovf > 0) ga[kk] += cur[slot * hw + q];
       }
-      {
-        const uint4 e0 = __ldg(ebp + 2 * q), e1 = __ldg(ebp + 2 * q + 1);
-        const uint32_t e[8] = {e0.x, e0.y, e0.z, e0.w, e1.x, e1.y, e1.z, e1.w};
+      const EllRow rb = ell_load_row(ebp, q);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          if (e[j] >> 16) {                                    // empty slots carry weight 0
-            const float wj = (float)(e[j] >> 16) * (1.0f / 65535.0f);
-            const int src = e[j] & 0xffffu;
+      for (int j = 0; j < 8; ++j) {
+        if (!ell_used(rb.e[j])) continue;
+        const float wj = ell_weight(rb.e[j]);
+        const int src = ell_source(rb.e[j]);
 #pragma unroll
-            for (int kk = 0; kk < KT; ++kk) ga[kk] = fmaf(-wj, __half2float(s1[(kk * G + g) * hw + src]), ga[kk]);
-          }
-        }
+        for (int kk = 0; kk < KT; ++kk) ga[kk] = fmaf(-wj, __half2float(s1[(kk * G + g) * hw + src]), ga[kk]);
       }
-      {
-        const uint4 e0 = __ldg(efp + 2 * q), e1 = __ldg(efp + 2 * q + 1);
-        const uint32_t e[8] = {e0.x, e0.y, e0.z, e0.w, e1.x, e1.y, e1.z, e1.w};
+      const EllRow rf = ell_load_row(efp, q);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          if (e[j] >> 16) {
-            const float wj = (float)(e[j] >> 16) * (1.0f / 65535.0f);
-            const int src = e[j] & 0xffffu;
+      for (int j = 0; j < 8; ++j) {
+        if (!ell_used(rf.e[j])) continue;
+        const float wj = ell_weight(rf.e[j]);
+        const int src = ell_source(rf.e[j]);
 #pragma unroll
-            for (int kk = 0; kk < KT; ++kk) gb[kk] = fmaf(-wj, __half2float(s2[(kk * G + g) * hw + src]), gb[kk]);
-          }
-        }
+        for (int kk = 0; kk < KT; ++kk) gb[kk] = fmaf(-wj, __half2float(s2[(kk * G + g) * hw + src]), gb[kk]);
       }
 #pragma unroll
       for (int kk = 0; kk < KT; ++kk) {
         if (own_live[kk]) {
           float* dst = grad + own_base[kk] + goff_a + q;
-          // frame f: this pair's term + its term as "next" of pair f-1.  Two rounded products and one add, never
-          // (carry + ga) * k: a frame-sharded batch adds the carry of a shard's first frame on the host (halo exchange)
-          // and must reproduce these bits
-          const float val = __fadd_rn(__fmul_rn(ga[kk], k), __fmul_rn(carry[pp * KT + kk], k));
+          const float val = grad_term(ga[kk], carry[pp * KT + kk], k);
           *dst = accumulate ? *dst + val : val;
         }
         carry[pp * KT + kk] = gb[kk];
@@ -939,12 +965,8 @@ warp_loss_group_kernel(const float* __restrict__ cs, const float* __restrict__ f
       const int32_t* of = ovf + ((long long)1 * frames + f) * n_ovf * 3;
       for (int e = t; e < n_ovf; e += T) {
         if (!ovf_run_head(of, e)) continue;
-        for (int slot = 0; slot < K; ++slot) {
-          float acc = 0.f;
-          for (int e2 = e; e2 < n_ovf && of[3 * e2] == of[3 * e]; ++e2)
-            acc = fmaf(-__int_as_float(of[3 * e2 + 2]), __half2float(s2[slot * hw + of[3 * e2 + 1]]), acc);
-          cur[slot * hw + of[3 * e]] = acc;
-        }
+        for (int slot = 0; slot < K; ++slot)
+          cur[slot * hw + of[3 * e]] = ovf_run_sum(of, n_ovf, e, [&](int src) { return __half2float(s2[slot * hw + src]); });
       }
       __syncthreads();
 #pragma unroll
@@ -970,23 +992,13 @@ warp_loss_group_kernel(const float* __restrict__ cs, const float* __restrict__ f
       if (own_live[kk]) {
         if (halo_grad != nullptr) {                            // open chain: the following rank's first frame receives it
           const int pl = blockIdx.x * K + kk * G + g;
-          halo_grad[((long long)(pl / channels) * channels + pl % channels) * hw + q] = __fmul_rn(carry[pp * KT + kk], k);
+          halo_grad[((long long)(pl / channels) * channels + pl % channels) * hw + q] = carry_term(carry[pp * KT + kk], k);
         } else {
-          grad[own_base[kk] + q] = __fadd_rn(grad[own_base[kk] + q], __fmul_rn(carry[pp * KT + kk], k));
+          grad[own_base[kk] + q] = add_carry(grad[own_base[kk] + q], carry[pp * KT + kk], k);
         }
       }
   }
-  if (loss_acc != nullptr) {
-    __shared__ float red[32];
-    loss = warp_sum(loss);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = loss;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      float v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
-      v = warp_sum(v);
-      if (threadIdx.x == 0) atomicAdd(loss_acc, v * k);
-    }
-  }
+  if (loss_acc != nullptr) cta_loss_add(loss, loss_acc, k);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1045,7 +1057,7 @@ warp_loss_quad_kernel(const float* __restrict__ cs, const float* __restrict__ fw
 
   load_frame(cur, 0);
   for (int f = 0; f < frames; ++f) {
-    const int fn = (f + 1 == frames) ? (halo_cs != nullptr ? frames : 0) : f + 1;
+    const int fn = next_frame(f, frames, halo_cs != nullptr);
     load_frame(nxt, fn);
     __syncthreads();
     // ---- residuals of pair (f, fn): taps and keep masks once per pixel, applied to the 4 NQ channels
@@ -1084,29 +1096,19 @@ warp_loss_quad_kernel(const float* __restrict__ cs, const float* __restrict__ fw
     }
     __syncthreads();
     // ---- destinations hit by more than 8 taps of the backward-flow warp: extra terms of d/dc1 (frame f) through the
-    //      dead frame-f planes; they join ga BEFORE it meets the carry (see warp_loss_group_kernel); run heads only, runs
-    //      summed in list order: no atomics, deterministic
+    //      dead frame-f planes; they join ga BEFORE it meets the carry (grad_term)
     if (n_ovf > 0) {
       for (int q = t; q < NQ * hw; q += T) cur[q] = make_float4(0.f, 0.f, 0.f, 0.f);
       __syncthreads();
       const int32_t* ob = ovf + ((long long)0 * frames + f) * n_ovf * 3;
       for (int e = t; e < n_ovf; e += T) {
         if (!ovf_run_head(ob, e)) continue;
-        for (int nq = 0; nq < NQ; ++nq) {
-          float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-          for (int e2 = e; e2 < n_ovf && ob[3 * e2] == ob[3 * e]; ++e2) {
-            const float wgt = -__int_as_float(ob[3 * e2 + 2]);
-            const float4 v = h4_to_f4(s1[nq * hw + ob[3 * e2 + 1]]);
-            acc.x = fmaf(wgt, v.x, acc.x), acc.y = fmaf(wgt, v.y, acc.y);
-            acc.z = fmaf(wgt, v.z, acc.z), acc.w = fmaf(wgt, v.w, acc.w);
-          }
-          cur[nq * hw + ob[3 * e]] = acc;
-        }
+        for (int nq = 0; nq < NQ; ++nq)
+          cur[nq * hw + ob[3 * e]] = ovf_run_sum(ob, n_ovf, e, [&](int src) { return h4_to_f4(s1[nq * hw + src]); });
       }
       __syncthreads();
     }
-    // ---- adjoints as gathers: 8 packed (source:u16, weight:unorm16) ELL slots per destination pixel, used slots first,
-    //      so a warp stops at the first slot that is empty for all of its lanes
+    // ---- adjoints as gathers through the ELL rows: a warp stops at the first slot that is unused in all of its lanes
     {
       const uint4* ebp = bwd_ell + (long long)f * hw * 2;
       const uint4* efp = fwd_ell + (long long)f * hw * 2;
@@ -1126,48 +1128,31 @@ warp_loss_quad_kernel(const float* __restrict__ cs, const float* __restrict__ fw
             ga[nq].x += o.x, ga[nq].y += o.y, ga[nq].z += o.z, ga[nq].w += o.w;
           }
         }
-        {
-          const uint4 e0 = __ldg(ebp + 2 * qq), e1 = __ldg(ebp + 2 * qq + 1);
-          const uint32_t e[8] = {e0.x, e0.y, e0.z, e0.w, e1.x, e1.y, e1.z, e1.w};
+        const EllRow rb = ell_load_row(ebp, qq);
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            if (!__any_sync(0xffffffffu, live && (e[j] >> 16) != 0)) break;
-            const float wj = -(float)(e[j] >> 16) * (1.0f / 65535.0f);
-            const int src = e[j] & 0xffffu;
+        for (int j = 0; j < 8; ++j) {
+          if (!__any_sync(0xffffffffu, live && ell_used(rb.e[j]))) break;
+          const float wj = -ell_weight(rb.e[j]);
+          const int src = ell_source(rb.e[j]);
 #pragma unroll
-            for (int nq = 0; nq < NQ; ++nq) {
-              const float4 v = h4_to_f4(s1[nq * hw + src]);
-              ga[nq].x = fmaf(wj, v.x, ga[nq].x), ga[nq].y = fmaf(wj, v.y, ga[nq].y);
-              ga[nq].z = fmaf(wj, v.z, ga[nq].z), ga[nq].w = fmaf(wj, v.w, ga[nq].w);
-            }
-          }
+          for (int nq = 0; nq < NQ; ++nq) ga[nq] = fma_acc(wj, h4_to_f4(s1[nq * hw + src]), ga[nq]);
         }
-        {
-          const uint4 e0 = __ldg(efp + 2 * qq), e1 = __ldg(efp + 2 * qq + 1);
-          const uint32_t e[8] = {e0.x, e0.y, e0.z, e0.w, e1.x, e1.y, e1.z, e1.w};
+        const EllRow rf = ell_load_row(efp, qq);
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            if (!__any_sync(0xffffffffu, live && (e[j] >> 16) != 0)) break;
-            const float wj = -(float)(e[j] >> 16) * (1.0f / 65535.0f);
-            const int src = e[j] & 0xffffu;
+        for (int j = 0; j < 8; ++j) {
+          if (!__any_sync(0xffffffffu, live && ell_used(rf.e[j]))) break;
+          const float wj = -ell_weight(rf.e[j]);
+          const int src = ell_source(rf.e[j]);
 #pragma unroll
-            for (int nq = 0; nq < NQ; ++nq) {
-              const float4 v = h4_to_f4(s2[nq * hw + src]);
-              gb[nq].x = fmaf(wj, v.x, gb[nq].x), gb[nq].y = fmaf(wj, v.y, gb[nq].y);
-              gb[nq].z = fmaf(wj, v.z, gb[nq].z), gb[nq].w = fmaf(wj, v.w, gb[nq].w);
-            }
-          }
+          for (int nq = 0; nq < NQ; ++nq) gb[nq] = fma_acc(wj, h4_to_f4(s2[nq * hw + src]), gb[nq]);
         }
 #pragma unroll
         for (int nq = 0; nq < NQ; ++nq) {
           if (live) {
             const float4 cr = carry[pp][nq];
             float* g4 = gdst + (long long)nq * 4 * hw;
-            // two rounded products and one add, never (carry + ga) * k (see warp_loss_group_kernel)
-            const float v0 = __fadd_rn(__fmul_rn(ga[nq].x, k), __fmul_rn(cr.x, k));
-            const float v1 = __fadd_rn(__fmul_rn(ga[nq].y, k), __fmul_rn(cr.y, k));
-            const float v2 = __fadd_rn(__fmul_rn(ga[nq].z, k), __fmul_rn(cr.z, k));
-            const float v3 = __fadd_rn(__fmul_rn(ga[nq].w, k), __fmul_rn(cr.w, k));
+            const float v0 = grad_term(ga[nq].x, cr.x, k), v1 = grad_term(ga[nq].y, cr.y, k);
+            const float v2 = grad_term(ga[nq].z, cr.z, k), v3 = grad_term(ga[nq].w, cr.w, k);
             if (accumulate) {
               g4[q] += v0, g4[hw + q] += v1, g4[2 * hw + q] += v2, g4[3 * hw + q] += v3;
             } else {
@@ -1186,16 +1171,8 @@ warp_loss_quad_kernel(const float* __restrict__ cs, const float* __restrict__ fw
       const int32_t* of = ovf + ((long long)1 * frames + f) * n_ovf * 3;
       for (int e = t; e < n_ovf; e += T) {
         if (!ovf_run_head(of, e)) continue;
-        for (int nq = 0; nq < NQ; ++nq) {
-          float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-          for (int e2 = e; e2 < n_ovf && of[3 * e2] == of[3 * e]; ++e2) {
-            const float wgt = -__int_as_float(of[3 * e2 + 2]);
-            const float4 v = h4_to_f4(s2[nq * hw + of[3 * e2 + 1]]);
-            acc.x = fmaf(wgt, v.x, acc.x), acc.y = fmaf(wgt, v.y, acc.y);
-            acc.z = fmaf(wgt, v.z, acc.z), acc.w = fmaf(wgt, v.w, acc.w);
-          }
-          cur[nq * hw + of[3 * e]] = acc;
-        }
+        for (int nq = 0; nq < NQ; ++nq)
+          cur[nq * hw + of[3 * e]] = ovf_run_sum(of, n_ovf, e, [&](int src) { return h4_to_f4(s2[nq * hw + src]); });
       }
       __syncthreads();
 #pragma unroll
@@ -1225,28 +1202,17 @@ warp_loss_quad_kernel(const float* __restrict__ cs, const float* __restrict__ fw
         const float4 cr = carry[pp][nq];
         if (halo_grad != nullptr) {                              // open chain: the following rank's first frame receives it
           float* g0 = halo_grad + halo_base + (long long)nq * 4 * hw;
-          g0[q] = __fmul_rn(cr.x, k), g0[hw + q] = __fmul_rn(cr.y, k);
-          g0[2 * hw + q] = __fmul_rn(cr.z, k), g0[3 * hw + q] = __fmul_rn(cr.w, k);
+          g0[q] = carry_term(cr.x, k), g0[hw + q] = carry_term(cr.y, k);
+          g0[2 * hw + q] = carry_term(cr.z, k), g0[3 * hw + q] = carry_term(cr.w, k);
         } else {
           float* g0 = grad + base + (long long)nq * 4 * hw;
-          g0[q] = __fadd_rn(g0[q], __fmul_rn(cr.x, k)), g0[hw + q] = __fadd_rn(g0[hw + q], __fmul_rn(cr.y, k));
-          g0[2 * hw + q] = __fadd_rn(g0[2 * hw + q], __fmul_rn(cr.z, k));
-          g0[3 * hw + q] = __fadd_rn(g0[3 * hw + q], __fmul_rn(cr.w, k));
+          g0[q] = add_carry(g0[q], cr.x, k), g0[hw + q] = add_carry(g0[hw + q], cr.y, k);
+          g0[2 * hw + q] = add_carry(g0[2 * hw + q], cr.z, k), g0[3 * hw + q] = add_carry(g0[3 * hw + q], cr.w, k);
         }
       }
     }
   }
-  if (loss_acc != nullptr) {
-    __shared__ float red[32];
-    loss = warp_sum(loss);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = loss;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      float v = threadIdx.x < ((blockDim.x + 31) >> 5) ? red[threadIdx.x] : 0.f;
-      v = warp_sum(v);
-      if (threadIdx.x == 0) atomicAdd(loss_acc, v * k);
-    }
-  }
+  if (loss_acc != nullptr) cta_loss_add(loss, loss_acc, k);
 }
 
 // =============================================================================================
