@@ -97,6 +97,26 @@ def adjoint_csr(flows, occs, size_h: int):
 
 
 # --------------------------------------------------------------------------- warp_tensor
+def chain_operands(flows, occs, saliency, n: int, h: int, w: int):
+    """The operands of warp_tensor's frame chain at an h x w feature map (src/flow_utils.py:24-51), cached per batch:
+    bwd_flow [n, 2, h, w], fwd_flow_last [2, h, w] and the blend weights [n, 1, h, w], all fp32."""
+    def prepare():
+        scale, fwd_flow, bwd_flow, fwd_occ, bwd_occ = resize_flows_occs(flows, occs, h)
+        if scale == 1:
+            bwd_occ = _dilate(bwd_occ, 13)
+            fwd_occ = _dilate(fwd_occ, 13)
+        scale2 = h * 1.0 / saliency.shape[2]
+        sal = F.interpolate(saliency.float(), scale_factor=scale2, mode="bilinear").contiguous()
+        warp_sal = ops.flow_warp(sal, bwd_flow)                                    # :38
+        warp_sal_last = ops.flow_warp(sal[0:1].contiguous(), fwd_flow[n - 1:n].contiguous())   # :39
+        blend = torch.empty(n, 1, h, w, dtype=torch.float32, device=bwd_flow.device)
+        blend[:n - 1] = (1 - bwd_occ[:n - 1]) * sal[1:n] * warp_sal[:n - 1]       # :45
+        blend[n - 1:] = (1 - fwd_occ[n - 1:n]) * sal[n - 1:n] * warp_sal_last      # :50
+        return bwd_flow, fwd_flow[n - 1].contiguous(), blend.contiguous()
+
+    return _cache_get(("warp_tensor", n, h, w), (flows[0], flows[1], occs[0], occs[1], saliency), prepare)
+
+
 @torch.no_grad()
 def warp_tensor(sample, flows, occs, saliency, unet_chunk_size, shard=None):
     """Warp + fuse along the frame chain (src/flow_utils.py:18-53).
@@ -115,22 +135,7 @@ def warp_tensor(sample, flows, occs, saliency, unet_chunk_size, shard=None):
     n = sample.shape[0] // unet_chunk_size if world == 1 else flows[0].shape[0]
     h, w = sample.shape[2], sample.shape[3]
 
-    def prepare():
-        scale, fwd_flow, bwd_flow, fwd_occ, bwd_occ = resize_flows_occs(flows, occs, h)
-        if scale == 1:
-            bwd_occ = _dilate(bwd_occ, 13)
-            fwd_occ = _dilate(fwd_occ, 13)
-        scale2 = h * 1.0 / saliency.shape[2]
-        sal = F.interpolate(saliency.float(), scale_factor=scale2, mode="bilinear").contiguous()
-        warp_sal = ops.flow_warp(sal, bwd_flow)                                    # :38
-        warp_sal_last = ops.flow_warp(sal[0:1].contiguous(), fwd_flow[n - 1:n].contiguous())   # :39
-        blend = torch.empty(n, 1, h, w, dtype=torch.float32, device=sample.device)
-        blend[:n - 1] = (1 - bwd_occ[:n - 1]) * sal[1:n] * warp_sal[:n - 1]       # :45
-        blend[n - 1:] = (1 - fwd_occ[n - 1:n]) * sal[n - 1:n] * warp_sal_last      # :50
-        return bwd_flow, fwd_flow[n - 1].contiguous(), blend.contiguous()
-
-    bwd_flow, fwd_flow_last, blend = _cache_get(("warp_tensor", n, h, w),
-                                                 (flows[0], flows[1], occs[0], occs[1], saliency), prepare)
+    bwd_flow, fwd_flow_last, blend = chain_operands(flows, occs, saliency, n, h, w)
 
     def chain(planes, chunks):
         return ops.warp_fuse_chain(planes, bwd_flow, fwd_flow_last, blend, chunks)

@@ -166,25 +166,63 @@ def temporal_attn_fwd(q_raw, k_raw, v_src, fwd_map, traj_mask, chunks: int, head
     return out
 
 
+def _check_warp_operands(what, specs):
+    """Refuse, before any launch, operands the warp kernels would misread: the C ABI takes raw pointers, so a wrong
+    dtype, shape or layout would be read as something else or out of bounds.  specs: (name, tensor, dtype, allowed
+    shapes); dtypes, shapes and layouts are checked first, then that every operand is a CUDA tensor on one device."""
+    for name, t, dtype, shapes in specs:
+        if not isinstance(t, torch.Tensor):
+            raise L.FrescoError(f"{what}: {name} must be a tensor")
+        if t.dtype != dtype:
+            raise L.FrescoError(f"{what}: {name} must be {dtype}, got {t.dtype}")
+        if tuple(t.shape) not in [tuple(s) for s in shapes]:
+            want = " or ".join(str(list(s)) for s in shapes)
+            raise L.FrescoError(f"{what}: {name} must have shape {want}, got {list(t.shape)}")
+        if not t.is_contiguous():
+            raise L.FrescoError(f"{what}: {name} must be contiguous")
+    dev = specs[0][1].device
+    for name, t, _, _ in specs:
+        if not t.is_cuda or t.device != dev:
+            raise L.FrescoError(f"{what}: {name} must be a CUDA tensor on the device of {specs[0][0]}, got {t.device}")
+
+
 def flow_warp(src: torch.Tensor, flow: torch.Tensor) -> torch.Tensor:
     """fp32 [B,C,h,w] warped by flow [Bf,2,h,w] (sample b uses flow b % Bf)."""
+    if not isinstance(src, torch.Tensor) or src.dim() != 4:
+        raise L.FrescoError("flow_warp: src must be fp32 [B, C, h, w]")
     B, C, h, w = src.shape
+    Bf = flow.shape[0] if isinstance(flow, torch.Tensor) and flow.dim() == 4 and flow.shape[0] > 0 else 1
+    _check_warp_operands("flow_warp", [("src", src, torch.float32, [src.shape]),
+                                       ("flow", flow, torch.float32, [(Bf, 2, h, w)])])
     dst = torch.empty_like(src)
-    L.check(L.lib().fresco_flow_warp(L.ptr(src), L.ptr(flow), L.ptr(dst), B, C, h, w, flow.shape[0], L.stream()),
+    L.check(L.lib().fresco_flow_warp(L.ptr(src), L.ptr(flow), L.ptr(dst), B, C, h, w, Bf, L.stream()),
             "fresco_flow_warp")
     return dst
 
 
 def warp_fuse_chain(sample, bwd_flow, fwd_flow_last, blend, chunks: int, out=None):
+    """sample fp16 / fp32 [chunks*N, C, h, w] (chunk-major); bwd_flow fp32 [N, 2, h, w]; fwd_flow_last fp32 [2, h, w];
+    blend fp32 [N, h, w] or [N, 1, h, w] -> out like sample (``out`` may be ``sample`` itself)."""
+    if not isinstance(sample, torch.Tensor) or sample.dim() != 4:
+        raise L.FrescoError("warp_fuse_chain: sample must be [chunks*frames, C, h, w]")
     B, C, h, w = sample.shape
+    if sample.dtype not in (torch.float16, torch.float32):
+        raise L.FrescoError("warp_fuse_chain: fp16 or fp32 only")
+    if not isinstance(chunks, int) or chunks <= 0 or B % chunks:
+        raise L.FrescoError(f"warp_fuse_chain: {B} planes do not split into {chunks} chunks")
+    n = B // chunks
+    specs = [("sample", sample, sample.dtype, [sample.shape]), ("bwd_flow", bwd_flow, torch.float32, [(n, 2, h, w)]),
+             ("fwd_flow_last", fwd_flow_last, torch.float32, [(2, h, w)]),
+             ("blend", blend, torch.float32, [(n, h, w), (n, 1, h, w)])]
+    if out is not None:
+        specs.append(("out", out, sample.dtype, [sample.shape]))
+    _check_warp_operands("warp_fuse_chain", specs)
     if out is None:
         out = torch.empty_like(sample)
     is_half = 1 if sample.dtype == torch.float16 else 0
-    if not is_half and sample.dtype != torch.float32:
-        raise L.FrescoError("warp_fuse_chain: fp16 or fp32 only")
     ev = _prof_begin()
     L.check(L.lib().fresco_warp_fuse_chain(L.ptr(sample), L.ptr(out), is_half, L.ptr(bwd_flow), L.ptr(fwd_flow_last),
-                                           L.ptr(blend), chunks, B // chunks, C, h, w, L.stream()),
+                                           L.ptr(blend), chunks, n, C, h, w, L.stream()),
             "fresco_warp_fuse_chain")
     # every frame read once and written once (SURVEY 8d counts 3 fp32 passes for the reference's unfused chain)
     _prof_end(ev, "warp_chain_C%d_%dx%d" % (C, h, w), 2.0 * sample.numel() * sample.element_size(), "hbm")

@@ -42,6 +42,48 @@ def test_argument_errors_do_not_touch_the_gpu(built_lib):
     assert rc == -1
 
 
+def test_warp_operand_errors_do_not_touch_the_gpu():
+    """ops.warp_fuse_chain and ops.flow_warp check every operand's dtype, shape and layout before the device, so each
+    mistake is refused with its own message (never read through a raw pointer), here on CPU tensors."""
+    from fresco_b200 import ops
+    from fresco_b200._lib import FrescoError
+    N, C, h, w = 3, 4, 6, 5
+    ok = {"sample": torch.zeros(2 * N, C, h, w), "bwd_flow": torch.zeros(N, 2, h, w),
+          "fwd_flow_last": torch.zeros(2, h, w), "blend": torch.zeros(N, 1, h, w)}
+    bad = [("sample", torch.zeros(2 * N, C, h, w, dtype=torch.float64), "fp16 or fp32"),
+           ("sample", torch.zeros(2 * N, C, h), "sample must be"),
+           ("sample", torch.zeros(2 * N, C, w, h).transpose(2, 3), "sample must be contiguous"),
+           ("bwd_flow", torch.zeros(N, 2, h, w, dtype=torch.float16), "bwd_flow must be torch.float32"),
+           ("bwd_flow", torch.zeros(N, h, w, 2), "bwd_flow must have shape"),
+           ("bwd_flow", torch.zeros(N + 1, 2, h, w), "bwd_flow must have shape"),
+           ("bwd_flow", torch.zeros(N, 2, w, h).transpose(2, 3), "bwd_flow must be contiguous"),
+           ("fwd_flow_last", torch.zeros(1, 2, h, w), "fwd_flow_last must have shape"),
+           ("blend", torch.zeros(N, 2, h, w), "blend must have shape"),
+           ("blend", torch.zeros(N, h, w, dtype=torch.float16), "blend must be torch.float32")]
+    for name, t, msg in bad:
+        args = dict(ok, **{name: t})
+        with pytest.raises(FrescoError, match=msg):
+            ops.warp_fuse_chain(args["sample"], args["bwd_flow"], args["fwd_flow_last"], args["blend"], 2)
+    with pytest.raises(FrescoError, match="do not split into 4 chunks"):
+        ops.warp_fuse_chain(ok["sample"], ok["bwd_flow"], ok["fwd_flow_last"], ok["blend"], 4)
+    for out, msg in ((torch.zeros(2 * N, C, h, w, dtype=torch.float16), "out must be torch.float32"),
+                     (torch.zeros(2 * N, C, h, w + 1), "out must have shape")):
+        with pytest.raises(FrescoError, match=msg):
+            ops.warp_fuse_chain(ok["sample"], ok["bwd_flow"], ok["fwd_flow_last"], ok["blend"], 2, out=out)
+    with pytest.raises(FrescoError, match="sample must be a CUDA tensor"):          # every operand right but the device
+        ops.warp_fuse_chain(ok["sample"], ok["bwd_flow"], ok["fwd_flow_last"], ok["blend"], 2)
+    src = torch.zeros(4, C, h, w)
+    for flow, msg in ((torch.zeros(2, 2, h, w, dtype=torch.float64), "flow must be torch.float32"),
+                      (torch.zeros(2, 2, h + 1, w), "flow must have shape"), (torch.zeros(2, h, w), "flow must have"),
+                      (torch.zeros(2, 2, w, h).transpose(2, 3), "flow must be contiguous")):
+        with pytest.raises(FrescoError, match=msg):
+            ops.flow_warp(src, flow)
+    with pytest.raises(FrescoError, match="src must be torch.float32"):
+        ops.flow_warp(src.half(), torch.zeros(2, 2, h, w))
+    with pytest.raises(FrescoError, match="src must be a CUDA tensor"):
+        ops.flow_warp(src, torch.zeros(2, 2, h, w))
+
+
 def test_default_attention_kernel_per_head_dim(built_lib):
     """Host-side kernel selection through the C ABI (no launch): the default variant per head_dim, the options select
     the other parity-tested variants, negative values restore the defaults, unknown names fail."""

@@ -11,7 +11,8 @@ the options, and the kernels the call must launch, in order, as ``fresco_last_ke
 * compares the output with a plain fp64 reference of the same operation, evaluated on the operands the kernel consumes
   (fp16-rounded where the kernel reads fp16).  The temporal-consistency loss rows are held elementwise to
   ``oracle.warp_loss_bound`` (``tests/test_gpu_warp_loss.py`` runs its input families on every loss kernel), the
-  temporal attention rows to ``oracle.temporal_bound`` (``tests/test_gpu_temporal_attention.py``).
+  temporal attention rows to ``oracle.temporal_bound`` (``tests/test_gpu_temporal_attention.py``), the warp-chain rows
+  to ``oracle.warp_chain_bound`` (``tests/test_gpu_warp_chain.py``).
 
 Instantiations no row reaches are listed with the reason in ``NOT_LAST`` (launched, but another kernel of the same
 call is what the record shows) or ``COVERED_ELSEWHERE`` (one instantiation per dtype, no selection; the named test
@@ -32,6 +33,7 @@ from oracle import attention_bound as AB
 from oracle import fresco_oracle as O
 from oracle import gmflow_bound as GB
 from oracle import temporal_bound as TB
+from oracle import warp_chain_bound as CB
 from oracle import warp_loss_bound as WB
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -328,42 +330,18 @@ row("loss-one-cta-6x4x100x100", ["warp_loss_kernel"], _warp_loss, N=3, C=4, h=10
 
 
 # ================================================================================================ warp chain
-def _chain_ref(sample, bwd, fwd_last, blend, chunks):
-    """The frame-chain loop of O.warp_tensor in fp64, with the per-pair blend weights given."""
-    B, C, h, w = sample.shape
-    n = B // chunks
-    z = sample.double().clone()
-    bf, ff, m = bwd.double(), fwd_last.double()[None], blend.double().reshape(n, 1, h, w)
-    for j in range(chunks):
-        base = n * j
-        for ii in range(n - 1):
-            warped = O.flow_warp(z[base + ii:base + ii + 1], bf[ii:ii + 1])
-            z[base + ii + 1] = z[base + ii + 1] * (1 - m[ii]) + warped[0] * m[ii]
-        warped = O.flow_warp(z[base:base + 1], ff)
-        z[base + n - 1] = z[base + n - 1] * (1 - m[n - 1]) + warped[0] * m[n - 1]
-    return z
-
-
 def _chain(fb, launch, chunks, N, C, h, w, dtype, seed=0):
-    """fresco_warp_fuse_chain.  Flows are multiples of 2^-10 px, so x + flow and the bilinear weights are exact in fp32
-    and the only fp32 rounding left is the blend arithmetic."""
-    g = torch.Generator(device="cuda").manual_seed(seed + C + h)
-    sample = torch.randn(chunks * N, C, h, w, device="cuda", generator=g).to(dtype)
-    bwd = (torch.randn(N, 2, h, w, device="cuda", generator=g) * 3 * 1024).round() / 1024
-    fwd_last = (torch.randn(2, h, w, device="cuda", generator=g) * 3 * 1024).round() / 1024
-    blend = torch.rand(N, h, w, device="cuda", generator=g)
+    """fresco_warp_fuse_chain on smooth non-dyadic flows (x + flow rounds in fp32, so the coordinate path real flows
+    take is exercised), fractional blend weights and values of 1e-3 and 1e3 in one plane: every element within oracle.warp_chain_bound of the fp64 chain;
+    tests/test_gpu_warp_chain.py runs the bound's input families on every chain kernel."""
+    d = CB.family("magnitudes", chunks, N, C, h, w, dtype=dtype, seed=seed + C + h, device="cuda")      # 1e-3 and 1e3
+    sample = d["sample"]
     out = torch.full_like(sample, float("nan"))
-    fb.ops.warp_fuse_chain(sample, bwd, fwd_last, blend, chunks, out=out)
+    fb.ops.warp_fuse_chain(sample, d["bwd"], d["fwd_last"], d["blend"], chunks, out=out)
     launch("fresco_warp_fuse_chain")
-    ref = _chain_ref(sample, bwd, fwd_last, blend, chunks)
-    o = out.double()
-    unwritten = (~torch.isfinite(o)).sum().item()
-    assert unwritten == 0, f"{unwritten} outputs not written"
-    scale = ref.abs().max().item()
-    # fp32: blend rounding; fp16: one ulp of the stored value (the fp32 chain value can round either way near a tie)
-    tol = 1e-5 * scale + (2.0 ** -10 * ref.abs() if dtype == torch.float16 else 0.0)
-    bad = (o - ref).abs() > tol
-    assert not bad.any(), f"{bad.sum().item()} elements off, max error {(o - ref).abs().max().item():.3g}"
+    ref, tol = CB.chain_reference_and_bound(sample, d["bwd"], d["fwd_last"], d["blend"], chunks)
+    ratio = CB.ratio(out, ref, tol)
+    assert not (ratio > 1).any(), "warp chain: " + _worst_tile(ratio.reshape(-1, h * w))
 
 
 def _chain_rejects_fp16_image_planes(fb, launch):
@@ -536,7 +514,8 @@ NOT_LAST = {
 }
 COVERED_ELSEWHERE = {
     "kv_compact_kernel": "test_gpu_kernels.py::test_kv_compact_bit_exact",
-    "flow_warp_kernel": "test_gpu_kernels.py::test_flow_warp_and_consistency",
+    "flow_warp_kernel": "test_gpu_warp_chain.py::test_flow_warp (within oracle.warp_chain_bound; also "
+                        "test_gpu_kernels.py::test_flow_warp_and_consistency)",
     "warp_taps_kernel": "test_gpu_warp_loss.py::test_warp_taps_bit_exact (and it builds the adjoint of every "
                         "temporal-loss row here)",
     "adam_kernel": "test_gpu_kernels.py::test_adam_matches_torch",

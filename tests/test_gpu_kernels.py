@@ -17,6 +17,7 @@ pytestmark = pytest.mark.gpu
 
 from oracle import fresco_oracle as O  # noqa: E402  (checker only)
 from oracle import temporal_bound as TB  # noqa: E402  (checker only)
+from oracle import warp_chain_bound as CB  # noqa: E402  (checker only)
 
 
 def T(a, device="cuda"):
@@ -215,40 +216,61 @@ def test_temporal_attention_vs_oracle(fb, golden):
 
 
 def test_flow_warp_and_consistency(fb, golden):
+    """The reference's geometry fixture: the fp64 warp on the fixture's operands reproduces the reference's fp32 output,
+    and the kernel is held to oracle.warp_chain_bound of that fp64 warp; the masks equal the fp64 masks wherever
+    |norm - thr| lies outside the band the warp bound implies, and equal the reference's masks there too."""
     g = golden("geometry")
     feat, bwd, fwd = T(g["feat"]), T(g["bwd"]), T(g["fwd"])
     w = fb.fu.flow_warp(feat, bwd)
-    assert (w.cpu() - T(g["warped"], "cpu")).abs().max().item() < 2e-5
+    ref, tol = CB.flow_warp_reference_and_bound(feat, bwd)
+    assert (ref - T(g["warped"]).double()).abs().max().item() < 2e-5        # the reference's grid_sample round trip
+    ratio = CB.ratio(w, ref, tol)
+    assert not (ratio > 1).any(), f"flow_warp: err/tol {ratio.max().item():.3g}"
     fo, bo = fb.fu.forward_backward_consistency_check(fwd, bwd)
-    # thresholded output: allow a handful of pixels sitting exactly on the threshold
-    assert (fo.cpu() != T(g["fwd_occ"], "cpu")).float().mean().item() < 1e-3
-    assert (bo.cpu() != T(g["bwd_occ"], "cpu")).float().mean().item() < 1e-3
+    m = CB.consistency_reference(fwd, bwd)
+    for name, got in (("fwd", fo), ("bwd", bo)):
+        want, band, theirs = m[name + "_occ"], m[name + "_band"], T(g[name + "_occ"]).bool()
+        assert not ((got.bool() != want) & ~band).any(), f"{name}_occ differs from fp64 outside the band"
+        assert not ((theirs != want) & ~band).any(), f"the reference's {name}_occ differs from fp64 outside the band"
+        assert band.sum().item() <= 1e-3 * band.numel(), band.sum().item()
+
+
+def _warp_tensor_within_bound(fb, sample, flows, occs, sal, chunks):
+    """warp_tensor, held to oracle.warp_chain_bound of the fp64 chain on the operands its own preparation made
+    (flow_utils.chain_operands).  Returns (out, the fp64 reference)."""
+    out = fb.fu.warp_tensor(sample, flows, occs, sal, chunks)
+    n, (h, w) = sample.shape[0] // chunks, sample.shape[2:]
+    bwd, fwd_last, blend = fb.fu.chain_operands(flows, occs, sal, n, h, w)
+    chain_in = sample if 2 * h * w * 4 <= 200 * 1024 else sample.float()         # image planes: the fp32 per-step kernel
+    ref, tol = CB.chain_reference_and_bound(chain_in, bwd, fwd_last, blend, chunks, out_dtype=sample.dtype)
+    ratio = CB.ratio(out, ref, tol)
+    assert out.dtype == sample.dtype and not (ratio > 1).any(), f"warp_tensor: err/tol {ratio.max().item():.3g}"
+    return out, ref
 
 
 def test_warp_tensor_golden(fb, golden):
+    """The fp64 chain on warp_tensor's prepared operands reproduces the reference's fp32 outputs (2e-5: its fp32
+    arithmetic), and warp_tensor is within the bound of that chain at fp32 and fp16."""
     g = golden("warp_tensor")
     flows = [T(g["fwd"]), T(g["bwd"])]
     occs = [T(g["fwd_occ"]), T(g["bwd_occ"])]
     sal = T(g["saliency"])
-    o = fb.fu.warp_tensor(T(g["sample_feat"]), flows, occs, sal, 2)
-    assert (o.cpu() - T(g["out_feat"], "cpu")).abs().max().item() < 2e-5
-    o = fb.fu.warp_tensor(T(g["sample_img"]), flows, occs, sal, 1)          # scale 1: dilation path
-    assert (o.cpu() - T(g["out_img"], "cpu")).abs().max().item() < 2e-5
-    # fp16 activations, as on the reference's GPU path
-    o16 = fb.fu.warp_tensor(T(g["sample_feat"]).half(), flows, occs, sal, 2)
-    assert o16.dtype == torch.float16
-    assert (o16.float().cpu() - T(g["out_feat"], "cpu")).abs().max().item() < 1e-2
+    _, ref = _warp_tensor_within_bound(fb, T(g["sample_feat"]), flows, occs, sal, 2)
+    assert (ref - T(g["out_feat"]).double()).abs().max().item() < 2e-5
+    _, ref = _warp_tensor_within_bound(fb, T(g["sample_img"]), flows, occs, sal, 1)          # scale 1: dilation path
+    assert (ref - T(g["out_img"]).double()).abs().max().item() < 2e-5
+    _warp_tensor_within_bound(fb, T(g["sample_feat"]).half(), flows, occs, sal, 2)   # fp16, as on the GPU path
 
 
 def test_warp_tensor_large_plane_path(fb):
-    """planes that do not fit shared memory (image resolution) use the per-step kernels"""
+    """planes that do not fit shared memory (image resolution) use the per-step kernels; the fp64 chain on the prepared
+    operands also matches the oracle's fp32 warp_tensor"""
     N, H, W = 3, 256, 256
     flows, occs = O.synth_flows(N, H, W, seed=4, mag=6.0)
     sal = torch.rand(N, 1, 128, 128, generator=torch.Generator().manual_seed(0))
     img = torch.randn(N, 3, H, W, generator=torch.Generator().manual_seed(1))
-    ref = O.warp_tensor(img, flows, occs, sal, 1)
-    out = fb.fu.warp_tensor(img.cuda(), [f.cuda() for f in flows], [o.cuda() for o in occs], sal.cuda(), 1)
-    assert (out.cpu() - ref).abs().max().item() < 5e-5
+    _, ref = _warp_tensor_within_bound(fb, img.cuda(), [f.cuda() for f in flows], [o.cuda() for o in occs], sal.cuda(), 1)
+    assert (ref.cpu() - O.warp_tensor(img, flows, occs, sal, 1).double()).abs().max().item() < 5e-5
 
 
 def test_warp_loss_forward_backward(fb, golden):

@@ -22,10 +22,24 @@ pytestmark = pytest.mark.gpu
 from oracle import attention_bound as AB  # noqa: E402  (checker only)
 from oracle import fresco_oracle as O  # noqa: E402  (checker only)
 from oracle import temporal_bound as TB  # noqa: E402  (checker only)
+from oracle import warp_chain_bound as CB  # noqa: E402  (checker only)
 
 
 def T(a, device="cuda"):
     return torch.from_numpy(np.asarray(a)).to(device)
+
+
+def _warp_tensor_within_bound(fb, sample, flows, occs, sal, chunks):
+    """warp_tensor, held to oracle.warp_chain_bound of the fp64 chain on the operands its own preparation made
+    (flow_utils.chain_operands).  Returns (out, the fp64 reference)."""
+    out = fb.fu.warp_tensor(sample, flows, occs, sal, chunks)
+    n, (h, w) = sample.shape[0] // chunks, sample.shape[2:]
+    bwd, fwd_last, blend = fb.fu.chain_operands(flows, occs, sal, n, h, w)
+    chain_in = sample if 2 * h * w * 4 <= 200 * 1024 else sample.float()         # image planes: the fp32 per-step kernel
+    ref, tol = CB.chain_reference_and_bound(chain_in, bwd, fwd_last, blend, chunks, out_dtype=sample.dtype)
+    ratio = CB.ratio(out, ref, tol)
+    assert out.dtype == sample.dtype and not (ratio > 1).any(), f"warp_tensor: err/tol {ratio.max().item():.3g}"
+    return out, ref
 
 
 @pytest.fixture(scope="module")
@@ -203,10 +217,10 @@ def test_set_b_through_the_kernels(fb, golden):
         # fp16 weights and activations through the 4 Linear layers (torch / cuBLAS) dominate this error, not the kernels
         assert (out - ref).abs().max().item() < 1e-2 * ref.abs().max().item(), flags
     flows, occs, sal = [T(g["fwd"]), T(g["bwd"])], [T(g["fwd_occ"]), T(g["bwd_occ"])], T(g["saliency"])
-    o = fb.fu.warp_tensor(T(g["sample_feat"]), flows, occs, sal, 2)
-    assert (o.cpu() - T(g["out_feat"], "cpu")).abs().max().item() < 2e-5
-    o = fb.fu.warp_tensor(T(g["sample_img"]), flows, occs, sal, 1)
-    assert (o.cpu() - T(g["out_img"], "cpu")).abs().max().item() < 2e-5
+    _, ref = _warp_tensor_within_bound(fb, T(g["sample_feat"]), flows, occs, sal, 2)
+    assert (ref - T(g["out_feat"]).double()).abs().max().item() < 2e-5         # the reference's fp32 arithmetic
+    _, ref = _warp_tensor_within_bound(fb, T(g["sample_img"]), flows, occs, sal, 1)
+    assert (ref - T(g["out_img"]).double()).abs().max().item() < 2e-5
     for tag, iters in (("full1", 1), ("full3", 3)):
         tr = fb.dh.OptimizeTrace()
         out = fb.dh.optimize_feature(T(g["opt_sample"]), flows, occs, correlation_matrix=[T(g["opt_target"])],
@@ -572,10 +586,8 @@ def test_warp_tensor_fp16_image_resolution(fb):
     flows, occs = O.synth_flows(N, H, W, seed=4, mag=6.0)
     sal = torch.rand(N, 1, H // 2, W // 2, generator=torch.Generator().manual_seed(0))
     img = torch.randn(N, 3, H, W, generator=torch.Generator().manual_seed(1)).half()
-    ref = O.warp_tensor(img.float(), flows, occs, sal, 1)
-    out = fb.fu.warp_tensor(img.cuda(), [f.cuda() for f in flows], [o.cuda() for o in occs], sal.cuda(), 1)
-    assert out.dtype == torch.float16
-    assert (out.float().cpu() - ref).abs().max().item() < 4e-3
+    _, ref = _warp_tensor_within_bound(fb, img.cuda(), [f.cuda() for f in flows], [o.cuda() for o in occs], sal.cuda(), 1)
+    assert (ref.cpu() - O.warp_tensor(img.float(), flows, occs, sal, 1).double()).abs().max().item() < 5e-5
 
 
 # ------------------------------------------------------------------------------------------------ GMFlow transformer rows
