@@ -178,6 +178,20 @@ class FRESCOAttnProcessor2_0:
         # optional frame sharding over the GPUs of one box: (world, rank, process_group); see fresco_b200/dist.py
         self.shard = shard
         self._sharded = None
+        self._layout = None
+
+    def set_batch_frames(self, n_frames: int) -> None:
+        """Tell a sharded processor the frame count of the keyframe batch it runs on (``inference`` and
+        ``get_intraframe_paras`` do): with fewer frames than ranks it holds one CFG half and exchanges within the ranks
+        of that half (``dist.shard_layout``).  Without a call, the frame layout is assumed."""
+        if self.shard is None:
+            return
+        from .dist import shard_layout
+        layout = shard_layout(n_frames, self.shard)
+        if layout.split_halves != (self._layout is not None and self._layout.split_halves) or (
+                layout.split_halves and (layout.world, layout.rank) != (self._layout.world, self._layout.rank)):
+            self._sharded = None
+        self._layout = layout
 
     def __call__(self, attn, hidden_states, encoder_hidden_states=None, attention_mask=None, temb=None):
         residual = hidden_states
@@ -237,8 +251,14 @@ class FRESCOAttnProcessor2_0:
         if self.shard is not None and ctrl is not None:
             if self._sharded is None:
                 from .dist import ShardedFRESCOAttention
-                world, rank, group = self.shard
-                self._sharded = ShardedFRESCOAttention(ctrl, world, rank, self.unet_chunk_size, group)
+                layout = self._layout
+                if layout is not None and layout.split_halves:
+                    # one CFG half: chunks = 1, the exchanges (and the no-mask frame-0 broadcast) within the half
+                    world, rank, group = layout.world, layout.rank, layout.group
+                    chunks = layout.chunks(self.unet_chunk_size)
+                else:
+                    (world, rank, group), chunks = self.shard, self.unet_chunk_size
+                self._sharded = ShardedFRESCOAttention(ctrl, world, rank, chunks, group)
             ref_q = ref_k = None
             if ctrl.use_intraattn:
                 ref = ctrl(None)
@@ -422,34 +442,52 @@ def optimize_feature(sample, flows, occs, correlation_matrix=[], intra_weight=1e
     if (not have_temporal) and (intra_weight == 0 or len(correlation_matrix) == 0):
         return sample
     be = backend if backend is not None else _OptKernels()
-    n = sample.shape[0] // unet_chunk_size
     _, C, h, w = sample.shape
     world = 1 if shard is None else int(shard[0])
-    comm = None
+    comm = loss_comm = None
+    split = False                       # this rank holds one CFG half (dist.shard_layout)
+    chunks = unet_chunk_size
+    n = sample.shape[0] // chunks
     lo, total = 0, n
+    mean_frames = None                  # total_frames of the temporal mean (None: this call's frames)
     if world > 1:
-        from .dist import RingComm, frame_range
+        from .dist import RingComm, shard_layout
         rank = int(shard[1])
         third = shard[2] if len(shard) > 2 else None
-        comm = third if hasattr(third, "shift") else RingComm(world, rank, third)
+        loss_comm = third if hasattr(third, "shift") else RingComm(world, rank, third)
         if flows is not None:
             total = int(flows[0].shape[0])
         else:
-            count = torch.full((1,), n, dtype=torch.int64, device=sample.device)
-            comm.all_reduce_sum(count)
-            total = int(count.item())
-        lo, hi = frame_range(total, world, rank)
-        if hi - lo != n:
-            raise FrescoError("optimize_feature: rank %d of %d owns frames [%d, %d) of the %d-frame batch, got %d"
-                              % (rank, world, lo, hi, total, n))
-    cs = sample.to(torch.float32).reshape(unet_chunk_size, n, C, h, w).contiguous().clone()
+            # every (chunk, frame) sample is held once in either layout: the batch has (all rows) / chunks frames
+            count = torch.full((1,), sample.shape[0], dtype=torch.int64, device=sample.device)
+            loss_comm.all_reduce_sum(count)
+            total = int(count.item()) // unet_chunk_size
+        layout = shard_layout(total, shard)
+        chunks = layout.chunks(unet_chunk_size)
+        n = sample.shape[0] // chunks
+        lo, hi = layout.lo, layout.hi
+        if hi - lo != n or sample.shape[0] != chunks * n:
+            raise FrescoError("optimize_feature: %r owns frames [%d, %d) of the %d-frame batch, got %d rows"
+                              % (layout, lo, hi, total, sample.shape[0]))
+        split = layout.split_halves
+        if split:
+            # the ring of this rank's CFG half; the loss trace still sums over the whole shard
+            sub = layout.group
+            comm = sub if hasattr(sub, "shift") else RingComm(layout.world, layout.rank, sub) if layout.world > 1 else None
+            # the halo kernel forms the mean's element count as chunks * total_frames * C*h*w in double: one chunk and
+            # 2N "frames" give the unsharded 2 * N * C*h*w exactly
+            mean_frames = 2 * total
+        else:
+            comm = loss_comm
+            mean_frames = total
+    cs = sample.to(torch.float32).reshape(chunks, n, C, h, w).contiguous().clone()
     grad = torch.empty_like(cs)
     exp_avg = torch.zeros_like(cs)
     exp_avg_sq = torch.zeros_like(cs)
     if have_temporal:
         prep = be.temporal_prepare(flows, occs, h, lo, lo + n, total)
         if comm is not None:
-            first, halo_cs, halo_grad, from_prev = (torch.empty(unet_chunk_size, C, h, w, dtype=torch.float32,
+            first, halo_cs, halo_grad, from_prev = (torch.empty(chunks, C, h, w, dtype=torch.float32,
                                                                 device=sample.device) for _ in range(4))
     target = None
     for tmp in correlation_matrix:
@@ -461,7 +499,11 @@ def optimize_feature(sample, flows, occs, correlation_matrix=[], intra_weight=1e
         target = target.to(torch.float32).contiguous()
     # F.l1_loss averages over the frames of the WHOLE batch: a rank's share of the weight, which the Gram kernels divide
     # by this rank's batch in double (ops.gram_*), so the fp32 loss scale is the unsharded one
-    weight = intra_weight * (float(n) / float(total))
+    # (a rank holding one CFG half has n of the 2N samples)
+    if split:
+        weight = intra_weight * (float(n) / float(2 * total))
+    else:
+        weight = intra_weight * (float(n) / float(total))
     loss_acc = torch.zeros(1, dtype=torch.float32, device=sample.device) if trace is not None else None
     for it in range(1, iters + 1):
         if loss_acc is not None:
@@ -469,22 +511,24 @@ def optimize_feature(sample, flows, occs, correlation_matrix=[], intra_weight=1e
         if have_temporal and comm is not None:
             first.copy_(cs[:, 0])
             comm.shift(first, halo_cs, -1)                      # my first frame is the previous rank's halo
-            be.temporal(cs, prep, grad, loss_acc, halo_cs, halo_grad, total)
+            be.temporal(cs, prep, grad, loss_acc, halo_cs, halo_grad, mean_frames)
             comm.shift(halo_grad, from_prev, +1)                # what my first frame receives from the previous rank's last pair
             grad[:, 0] += from_prev
+        elif have_temporal and mean_frames is not None:
+            be.temporal(cs, prep, grad, loss_acc, total_frames=mean_frames)     # one CFG half on a one-rank half group
         elif have_temporal:
             be.temporal(cs, prep, grad, loss_acc)
         else:
             grad.zero_()
         if spatial:
-            be.spatial(cs.view(unet_chunk_size * n, C, h * w), target, weight, grad.view(unet_chunk_size * n, C, h * w),
+            be.spatial(cs.view(chunks * n, C, h * w), target, weight, grad.view(chunks * n, C, h * w),
                        loss_acc)
         be.adam(cs, grad, exp_avg, exp_avg_sq, it)
         if trace is not None:
-            if comm is not None:
-                comm.all_reduce_sum(loss_acc)
+            if loss_comm is not None:
+                loss_comm.all_reduce_sum(loss_acc)
             trace.losses.append(float(loss_acc.item()))
-    return be.adain(cs.view(unet_chunk_size * n, C, h, w), sample)
+    return be.adain(cs.view(chunks * n, C, h, w), sample)
 
 
 def my_forward(self, steps=[], layers=[0, 1, 2, 3], flows=None, occs=None, correlation_matrix=[],
@@ -607,14 +651,23 @@ def get_intraframe_paras(pipe, imgs, frescoProc, prompt_embeds, do_classifier_fr
     initial noise is drawn for all of them from the seeded generator and this rank's frames [rank*N//G, (rank+1)*N//G)
     are sliced, encoded and run through the store pass.  The controller then holds this rank's reference inputs and
     the targets cover this rank's frames (both CFG chunks): what the sharded processor and
-    ``optimize_feature(shard=...)`` take.  The pass is per frame, so no collective is issued."""
-    from .dist import chunk_frames, shard_frames
+    ``optimize_feature(shard=...)`` take.  The pass is per frame, so no collective is issued.  With fewer frames than
+    ranks (``dist.shard_layout``'s half layout) the pass runs on this rank's CFG half only, the targets cover its
+    samples, and the VAE posterior sample is drawn on the half-0 rank and sent to its partner."""
+    from .dist import partner_share, shard_layout
     scheduler = pipe.scheduler
     timestep = scheduler.timesteps[-1]
     device = pipe._execution_device
     generator = torch.Generator(device=device).manual_seed(seed)
     B, C, H, W = imgs.shape
-    lo, hi = shard_frames(B, shard)
+    layout = shard_layout(B, shard)
+    lo, hi = (0, B) if layout is None else (layout.lo, layout.hi)
+    split = layout is not None and layout.split_halves
+    chunks = 2 if do_classifier_free_guidance else 1
+    if split:
+        layout.chunks(chunks)                                       # the half layout needs both CFG halves
+    if hasattr(frescoProc, "set_batch_frames"):
+        frescoProc.set_batch_frames(B)
     ctrl = frescoProc.controller
     ctrl.disable_controller()
     disable_FRESCO_opt(pipe)
@@ -622,12 +675,15 @@ def get_intraframe_paras(pipe, imgs, frescoProc, prompt_embeds, do_classifier_fr
     ctrl.enable_store()
     latents = pipe.prepare_latents(B, pipe.unet.config.in_channels, H, W, prompt_embeds.dtype, device, generator,
                                    latents=None)[lo:hi]             # all N frames: same Philox stream on every rank
-    latent_x0 = pipe.vae.config.scaling_factor * pipe.vae.encode(imgs[lo:hi].to(pipe.unet.dtype)).latent_dist.sample()
+
+    def encode():
+        return pipe.vae.config.scaling_factor * pipe.vae.encode(imgs[lo:hi].to(pipe.unet.dtype)).latent_dist.sample()
+    latent_x0 = (partner_share(layout, encode, (latents.shape, getattr(pipe.vae, "dtype", pipe.unet.dtype), latents.device))
+                 if split else encode())
     latents = scheduler.add_noise(latent_x0, latents, timestep).detach()
-    chunks = 2 if do_classifier_free_guidance else 1
-    model_in = torch.cat([latents] * 2) if do_classifier_free_guidance else latents
-    out = pipe.unet(model_in, timestep, encoder_hidden_states=chunk_frames(prompt_embeds, chunks, B, lo, hi),
-                    cross_attention_kwargs=None, return_dict=False)
+    model_in = torch.cat([latents] * 2) if do_classifier_free_guidance and not split else latents
+    pe = prompt_embeds if layout is None else layout.rows(prompt_embeds, chunks)
+    out = pipe.unet(model_in, timestep, encoder_hidden_states=pe, cross_attention_kwargs=None, return_dict=False)
     ctrl.disable_store()
     return gram_targets(out[1:])
 
@@ -643,19 +699,32 @@ def get_flow_and_interframe_paras(flow_model, imgs, visualize_pipeline=False, sh
     ``shard=(world, rank[, group])`` (not in the reference): every rank gets all N frames, runs GMFlow on its own
     pairs ``frame_range(N, world, rank)`` only and one all-gather (blocks padded to the largest share) assembles the
     whole batch's flows (rank order == pair order).  Occlusions, masks and trajectories are then built from the gathered flows on every rank, as unsharded:
-    the return values are the whole batch's, as in the unsharded call."""
-    from .dist import all_gather_frames, shard_frames
+    the return values are the whole batch's, as in the unsharded call.  With fewer frames than ranks
+    (``dist.shard_layout``'s half layout) the ranks of half 0 compute every pair once and each sends the gathered
+    flows to its partner: GMFlow is a network outside this library, whose bits could differ between two devices."""
+    from .dist import all_gather_frames, layout_group, partner_share, shard_layout
     from .flow_utils import flow_warp, forward_backward_consistency_check, get_mapping_ind
-    dev = next(flow_model.parameters()).device
+    param = next(flow_model.parameters())
+    dev = param.device
     images = torch.stack([torch.from_numpy(im).permute(2, 0, 1).float() for im in imgs], dim=0).to(dev)
     imgs_torch = images / 127.5 - 1.0                                   # numpy2tensor (src/utils.py:8-12)
     reshuffle = list(range(1, len(images))) + [0]
-    lo, hi = shard_frames(len(images), shard)
-    res = flow_model(images[lo:hi], images[reshuffle][lo:hi], attn_splits_list=[2], corr_radius_list=[-1],
-                     prop_radius_list=[-1], pred_bidir_flow=True)
-    flow = res["flow_preds"][-1]                                        # [2 * pairs, 2, H, W]: forward | backward
-    if shard is not None and shard[0] > 1:
-        flow = all_gather_frames(flow, len(images), shard[0], 2, shard[2] if len(shard) > 2 else None)
+    n = len(images)
+    layout = shard_layout(n, shard)
+    lo, hi = (0, n) if layout is None else (layout.lo, layout.hi)
+
+    def flows():
+        res = flow_model(images[lo:hi], images[reshuffle][lo:hi], attn_splits_list=[2], corr_radius_list=[-1],
+                         prop_radius_list=[-1], pred_bidir_flow=True)
+        flow = res["flow_preds"][-1]                                    # [2 * pairs, 2, H, W]: forward | backward
+        grp = layout_group(layout)
+        if grp is not None:
+            flow = all_gather_frames(flow, n, grp[0], 2, grp[2])
+        return flow
+    if layout is not None and layout.split_halves:
+        flow = partner_share(layout, flows, ((2 * n, 2) + tuple(images.shape[2:]), param.dtype, dev))
+    else:
+        flow = flows()
     fwd_flows, bwd_flows = flow.chunk(2)
     fwd_flows, bwd_flows = fwd_flows.contiguous(), bwd_flows.contiguous()
     fwd_occs, bwd_occs = forward_backward_consistency_check(fwd_flows, bwd_flows)

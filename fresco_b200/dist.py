@@ -2,8 +2,9 @@
 
 The reference has no collective on this path (SURVEY 2.1); this module is the multi-GPU design for BASELINE config 4: the
 N keyframes of ONE batch are split contiguously over G ranks (rank r owns frames ``frame_range(N, G, r)`` =
-[r*N//G, (r+1)*N//G) of both CFG chunks; G need not divide N) and the UNet body runs as plain replicas.  Only FRESCO
-attention couples frames:
+[r*N//G, (r+1)*N//G) of both CFG chunks; G need not divide N) and the UNet body runs as plain replicas.  A batch of
+G/2 <= N < G frames on an even G is split over the two CFG halves as well (``shard_layout``): every exchange below then
+runs with one chunk within the ranks of a half.  Only FRESCO attention couples frames:
 
 * cross-frame attention (src/diffusion_hacked.py:225-247, :303-305): every query frame attends the same K/V set = all
   tokens of frame 0 + the occluded tokens of frames 1..N-1.  Each rank compacts the selected rows of ITS frames straight
@@ -46,9 +47,170 @@ def block_sizes(n_frames: int, world: int) -> List[int]:
     return [hi - lo for lo, hi in (frame_range(n_frames, world, r) for r in range(world))]
 
 
-def shard_frames(n_frames: int, shard) -> Tuple[int, int]:
-    """frame range [lo, hi) of this rank for ``shard=(world, rank[, group])``; the whole batch for ``shard=None``"""
-    return (0, n_frames) if shard is None else frame_range(n_frames, shard[0], shard[1])
+class ShardLayout:
+    """What one rank of a sharded keyframe batch holds and whom it exchanges with (``shard_layout``).
+
+    ``halves`` = [h0, h1): the CFG halves (0 unconditional, 1 text) of frames [``lo``, ``hi``) this rank holds.
+    ``world`` / ``rank`` / ``group``: the process group the frame-sharded exchanges (K/V all-gather, trajectory
+    all-to-alls, ring halo, warp re-shard, frame gathers) run on.  ``partner``: the global rank holding the other half
+    of the same frames, or None.  ``shard`` is the ``(world, rank, group)`` the caller passed."""
+
+    def __init__(self, n_frames, halves, lo, hi, world, rank, group, partner, shard):
+        self.n_frames, self.halves, self.lo, self.hi = n_frames, halves, lo, hi
+        self.world, self.rank, self.group, self.partner, self.shard = world, rank, group, partner, shard
+
+    @property
+    def split_halves(self) -> bool:
+        return self.partner is not None
+
+    @property
+    def half(self) -> int:
+        """the CFG half this rank holds in the half layout"""
+        return self.halves[0]
+
+    def chunks(self, cfg_chunks: int) -> int:
+        """CFG chunks of this rank's rows for a call that would hold ``cfg_chunks`` unsharded"""
+        if not self.split_halves:
+            return cfg_chunks
+        if cfg_chunks != 2:
+            raise ValueError(f"{self.n_frames} frames on {self.shard[0]} ranks shard over the two classifier-free "
+                             f"guidance halves, so the batch needs both (got {cfg_chunks} chunk)")
+        return 1
+
+    def rows(self, t: Optional[torch.Tensor], cfg_chunks: int) -> Optional[torch.Tensor]:
+        """this rank's rows of a ``(chunk, frame)``-major batch ``[cfg_chunks * N, ...]`` (prompt embeddings, ControlNet
+        edges, Gram targets): frames [lo, hi) of each chunk it holds.  Anything not laid out that way comes back as it
+        is (see ``chunk_frames``)."""
+        if not self.split_halves:
+            return chunk_frames(t, cfg_chunks, self.n_frames, self.lo, self.hi)
+        if t is None or t.shape[0] != 2 * self.n_frames:
+            return t
+        base = self.half * self.n_frames
+        return t[base + self.lo:base + self.hi]
+
+    def __repr__(self):
+        return (f"ShardLayout(n_frames={self.n_frames}, halves={self.halves}, frames=[{self.lo}, {self.hi}), "
+                f"world={self.world}, rank={self.rank}, partner={self.partner})")
+
+
+_HALF_GROUPS: dict = {}
+
+
+def _global_rank(group, r: int) -> int:
+    return dist.get_global_rank(group, r) if group is not None else r
+
+
+def _splits_nccl(group) -> bool:
+    """True when a new NCCL group would be split from the default group's communicator: the default group is
+    bound to a device (``init_process_group(..., device_id=...)``), and ``ncclCommSplit`` is collective over every rank
+    of the communicator it splits"""
+    return bool(getattr(dist.group.WORLD, "bound_device_id", None)) and dist.get_backend(group) == dist.Backend.NCCL
+
+
+def half_group(world: int, rank: int, group=None):
+    """The process group of the CFG half of rank ``rank`` of the shard group ``group`` (``world`` ranks): group ranks
+    [h*G/2, (h+1)*G/2) for h = rank // (G/2).  It depends on G and the shard's ranks only, is created on the first call
+    (every rank of the shard reaches its first half-layout entry point in the same order) and cached by the global
+    ranks of the shard, so a shard group made again over the same ranks finds it.  Only the shard's ranks take part:
+    under NCCL with a device-bound default group the shard group is split in two (``split_group``, collective over the
+    shard's ranks only: a plain ``new_group`` would split the default communicator, which needs every rank of the
+    world); otherwise each half is created by its own ranks (``new_group(..., use_local_synchronization=True)``)."""
+    per = world // 2
+    shard_ranks = tuple(_global_rank(group, r) for r in range(world))
+    if shard_ranks in _HALF_GROUPS:
+        return _HALF_GROUPS[shard_ranks]
+    if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
+        raise RuntimeError("the CFG-half process groups must exist before a step is captured: call a sharded entry "
+                           "point (get_flow_and_interframe_paras, get_intraframe_paras, inference) first")
+    if per == 1:
+        sub = None
+    elif _splits_nccl(group):
+        sub = dist.split_group(parent_pg=group, split_ranks=[list(range(per)), list(range(per, world))])
+    else:
+        h = rank // per
+        sub = dist.new_group(list(shard_ranks[h * per:(h + 1) * per]), use_local_synchronization=True)
+    _HALF_GROUPS[shard_ranks] = sub
+    return sub
+
+
+def shard_layout(n_frames: int, shard) -> Optional[ShardLayout]:
+    """The partition of a keyframe batch of ``n_frames`` frames (2N samples: an unconditional and a text half) over
+    ``shard=(world, rank[, group])``; None for ``shard=None``.  Chosen by shape alone:
+
+    * N >= G: the frame layout -- rank r holds both halves of frames ``frame_range(N, G, r)``, the exchanges run on
+      ``group``.
+    * G even and G/2 <= N < G: the half layout -- rank r holds half r // (G/2) of frames ``frame_range(N, G/2, r %
+      (G/2))``; the exchanges run on the group of its half (``half_group``); its partner r +- G/2 holds the other half
+      of the same frames.
+    * otherwise: ValueError."""
+    if shard is None:
+        return None
+    if isinstance(shard, ShardLayout):
+        return shard
+    world, rank = int(shard[0]), int(shard[1])
+    group = shard[2] if len(shard) > 2 else None
+    if n_frames >= world:
+        lo, hi = frame_range(n_frames, world, rank)
+        return ShardLayout(n_frames, (0, 2), lo, hi, world, rank, group, None, shard)
+    if world % 2 != 0 or 2 * n_frames < world:
+        raise ValueError(f"{n_frames} frames cannot be sharded over {world} ranks: shard over the two guidance halves "
+                         f"needs an even number of ranks G <= 2N = {2 * n_frames}, or run the batch on a process group "
+                         f"of {n_frames} ranks, shard=({n_frames}, rank, group)")
+    per = world // 2
+    h, r = rank // per, rank % per
+    lo, hi = frame_range(n_frames, per, r)
+    if hasattr(group, "half_comm"):
+        # an injected communicator (tests: ranks as threads) supplies the communicator of the half itself
+        sub, partner = group.half_comm(world, rank), (1 - h) * per + r
+    else:
+        sub, partner = half_group(world, rank, group), _global_rank(group, (1 - h) * per + r)
+    return ShardLayout(n_frames, (h, h + 1), lo, hi, per, r, sub, partner, shard)
+
+
+def layout_group(layout: Optional[ShardLayout]):
+    """(world, rank, group) of the exchanges of ``layout``, as ``shard`` takes them; None when nothing is exchanged"""
+    if layout is None or layout.world == 1:
+        return None
+    return (layout.world, layout.rank, layout.group)
+
+
+def send_recv(sends, recvs, group=None) -> None:
+    """One batched point-to-point exchange: ``sends`` / ``recvs`` are lists of (tensor, global peer rank).  Under
+    NCCL it runs on the current stream with no host synchronisation; gloo moves host memory only, so GPU tensors are
+    staged through host copies there."""
+    stage = dist.get_backend(group) == dist.Backend.GLOO and any(t.is_cuda for t, _ in list(sends) + list(recvs))
+    out = [(torch.empty(t.shape, dtype=t.dtype) if stage else t, p) for t, p in recvs]
+    ops = ([dist.P2POp(dist.isend, t.cpu() if stage else t, p, group) for t, p in sends]
+           + [dist.P2POp(dist.irecv, t, p, group) for t, p in out])
+    for r in dist.batch_isend_irecv(ops):
+        r.wait()
+    if stage:
+        for (dst, _), (src, _) in zip(recvs, out):
+            dst.copy_(src)
+
+
+def partner_swap(layout: ShardLayout, mine: torch.Tensor) -> torch.Tensor:
+    """The partner's tensor of the same shape and dtype as ``mine``: one batched send / receive pair (``send_recv``,
+    as ``RingComm.shift``)."""
+    mine = mine.contiguous()
+    theirs = torch.empty_like(mine)
+    send_recv([(mine, layout.partner)], [(theirs, layout.partner)], layout.shard[2] if len(layout.shard) > 2 else None)
+    return theirs
+
+
+def partner_share(layout: ShardLayout, make, like: Tuple[tuple, torch.dtype, torch.device]) -> torch.Tensor:
+    """What ``make()`` returns, computed once on the half-0 rank and sent to its partner, which receives it into a
+    tensor of ``like = (shape, dtype, device)`` without calling ``make``.  Used for everything drawn from an unseeded
+    generator or computed by a network outside this library, whose bits could differ between two devices."""
+    group = layout.shard[2] if len(layout.shard) > 2 else None
+    if layout.half == 0:
+        out = make().contiguous()
+        send_recv([(out, layout.partner)], [], group)
+    else:
+        shape, dtype, device = like
+        out = torch.empty(shape, dtype=dtype, device=device)
+        send_recv([], [(out, layout.partner)], group)
+    return out
 
 
 def chunk_frames(t: Optional[torch.Tensor], chunks: int, n_frames: int, lo: int, hi: int) -> Optional[torch.Tensor]:
@@ -101,10 +263,7 @@ class RingComm:
 
     def shift(self, send: torch.Tensor, recv: torch.Tensor, direction: int) -> None:
         dst, src = self._peer(self.rank + direction), self._peer(self.rank - direction)
-        reqs = dist.batch_isend_irecv([dist.P2POp(dist.isend, send, dst, self.group),
-                                       dist.P2POp(dist.irecv, recv, src, self.group)])
-        for r in reqs:
-            r.wait()
+        send_recv([(send, dst)], [(recv, src)], self.group)
 
     def all_reduce_sum(self, t: torch.Tensor) -> None:
         dist.all_reduce(t, group=self.group)

@@ -125,14 +125,27 @@ def warp_tensor(sample, flows, occs, saliency, unet_chunk_size, shard=None):
     modifies ``sample``; the result has the dtype of ``sample``.
 
     ``shard=(world, rank[, group])`` (not in the reference): ``sample`` holds this rank's frames of a frame-sharded
-    batch (flows / occs / saliency describe ALL N frames).  The chain is sequential over frames but independent per
-    (chunk, channel) plane, so the batch is re-sharded by CHANNEL for the chain: one all-to-all turns
+    batch (flows / occs / saliency describe ALL N frames).  With fewer frames than ranks (``dist.shard_layout``'s half
+    layout) ``sample`` holds one CFG half of this rank's frames, [n_local, ...] whatever ``unet_chunk_size`` says,
+    and everything below runs within the ranks of that half (``shard`` may also be the ``ShardLayout`` itself).  The
+    chain is sequential over frames but independent per (chunk, channel) plane, so the batch is re-sharded by CHANNEL
+    for the chain: one all-to-all turns
     [frames/G, all channels] into [all frames, channels/G], every rank runs the chain kernel on its channel slice, a
     second all-to-all brings the frames back (SURVEY 8e, "sequential pieces").  When the channels do not split over the
     ranks (a decoded image has 3: background smoothing, src/pipe_FRESCO.py:46) every rank all-gathers the frames instead,
     runs the chain on the whole batch and keeps its own frames."""
-    world = 1 if shard is None else shard[0]
-    n = sample.shape[0] // unet_chunk_size if world == 1 else flows[0].shape[0]
+    layout = None
+    if shard is not None:
+        from .dist import shard_layout
+        layout = shard_layout(flows[0].shape[0], shard)
+        if layout.world == 1 and not layout.split_halves:
+            layout = None                                       # one rank: the unsharded call
+    world = 1 if layout is None else layout.world
+    if layout is not None and layout.split_halves:
+        # one CFG half (or, in background smoothing, the decoded frames on the ranks of half 0): one chunk, the
+        # exchanges within the ranks of the half
+        unet_chunk_size = 1
+    n = sample.shape[0] // unet_chunk_size if layout is None else flows[0].shape[0]
     h, w = sample.shape[2], sample.shape[3]
 
     bwd_flow, fwd_flow_last, blend = chain_operands(flows, occs, saliency, n, h, w)
@@ -149,15 +162,17 @@ def warp_tensor(sample, flows, occs, saliency, unet_chunk_size, shard=None):
         return t
 
     if world == 1:
+        if layout is not None and sample.shape[0] != n:
+            raise ValueError(f"warp_tensor: one CFG half of {n} frames needs {n} planes, got {sample.shape[0]}")
         return chain(chain_input(sample.contiguous()), unet_chunk_size).to(sample.dtype)
     import torch.distributed as dist
-    from .dist import all_gather_frames, block_sizes, frame_range
-    group = shard[2] if len(shard) > 2 else None
+    from .dist import all_gather_frames, block_sizes
+    group, rank = layout.group, layout.rank
     chunks, C = unet_chunk_size, sample.shape[1]
-    lo, hi = frame_range(n, world, shard[1])
+    lo, hi = layout.lo, layout.hi
     n_local = hi - lo
     if sample.shape[0] != chunks * n_local:
-        raise ValueError(f"warp_tensor: rank {shard[1]} of {world} owns frames [{lo}, {hi}) of {n}, "
+        raise ValueError(f"warp_tensor: rank {rank} of {world} owns frames [{lo}, {hi}) of {n}, "
                          f"so sample needs {chunks * n_local} planes, got {sample.shape[0]}")
     if C % world != 0:
         # gather path: the frames travel in the dtype of ``sample`` (fp16 VAE output: 1.5 MB per 512^2 frame), the chain

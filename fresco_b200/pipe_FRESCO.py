@@ -22,7 +22,7 @@ from typing import List, Optional
 import torch
 
 from . import ops
-from .dist import chunk_frames, shard_frames
+from .dist import layout_group, partner_share, partner_swap, shard_layout
 from .flow_utils import warp_tensor
 
 
@@ -52,16 +52,32 @@ def step(pipe, model_output, timestep, sample, generator, repeat_noise=False, vi
     ``noise`` (optional) replaces the ``torch.randn`` draw of :61-62 (the frame-sharded loop passes its slice).
     ``shard=(world, rank[, group])``: ``sample`` holds this rank's frames of a frame-sharded batch (``flows`` / ``occs``
     / ``saliency`` the whole batch's); background smoothing decodes and re-encodes those frames only and warps them
-    along the whole chain."""
+    along the whole chain.  ``shard`` may be a ``dist.ShardLayout``; in its half layout ``model_output`` is this rank's
+    CFG half of the raw UNet output [n, ...]: it is swapped with the partner's (one send / receive pair) so both run the
+    guidance on the same [uncond; text] operands, and the smoothing round trip runs on the ranks of half 0, which send
+    its result to their partners."""
     alpha_prod_t, c_x0, c_xt, sigma = _step_coefficients(pipe.scheduler, timestep)
     sample = sample.contiguous()
     do_cfg = guidance_scale is not None
+    layout = shard if hasattr(shard, "split_halves") and shard.split_halves else None
+    if layout is not None:
+        if not do_cfg:
+            raise ValueError("a batch sharded over the CFG halves needs guidance_scale")
+        mine = model_output.contiguous()
+        theirs = partner_swap(layout, mine)
+        model_output = torch.cat([mine, theirs] if layout.half == 0 else [theirs, mine])
     pred_original_sample = ops.cfg_pred_x0(model_output.contiguous(), sample, guidance_scale if do_cfg else 0.0,
                                            alpha_prod_t, do_cfg=do_cfg)
     if saliency is not None and flows is not None and occs is not None:                        # :44-47
-        image = pipe.vae.decode(pred_original_sample / pipe.vae.config.scaling_factor).sample
-        image = warp_tensor(image, flows, occs, saliency, unet_chunk_size=1, shard=shard)
-        pred_original_sample = (pipe.vae.config.scaling_factor * pipe.vae.encode(image).latent_dist.sample()).contiguous()
+        def smooth():
+            image = pipe.vae.decode(pred_original_sample / pipe.vae.config.scaling_factor).sample
+            image = warp_tensor(image, flows, occs, saliency, unet_chunk_size=1, shard=shard)
+            return (pipe.vae.config.scaling_factor * pipe.vae.encode(image).latent_dist.sample()).contiguous()
+        if layout is None:
+            pred_original_sample = smooth()
+        else:
+            pred_original_sample = partner_share(layout, smooth, (pred_original_sample.shape, pred_original_sample.dtype,
+                                                                  pred_original_sample.device))
     if noise is None:
         noise = torch.randn(sample.shape, generator=generator, device=sample.device, dtype=sample.dtype)
     pred_prev_sample = ops.ddpm_prev(pred_original_sample, sample, noise.contiguous(), c_x0, c_xt, sigma,
@@ -96,7 +112,11 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
     noise_scheduler = pipe.scheduler
     generator = torch.Generator(device=device).manual_seed(seed)
     B, C, H, W = imgs.shape
-    lo, hi = shard_frames(B, shard)
+    layout = shard_layout(B, shard)
+    lo, hi = (0, B) if layout is None else (layout.lo, layout.hi)
+    split = layout is not None and layout.split_halves
+    if hasattr(frescoProc, "set_batch_frames"):
+        frescoProc.set_batch_frames(B)
     latents = pipe.prepare_latents(B, pipe.unet.config.in_channels, H, W, prompt_embeds.dtype, device, generator,
                                    latents=None)                                # all N frames: same Philox stream everywhere
     if repeat_noise:
@@ -105,11 +125,18 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
         latents_init = latents.detach()[lo:hi]
         num_warmup_steps = 0
     else:
-        latent_x0 = pipe.vae.config.scaling_factor * pipe.vae.encode(imgs[lo:hi].to(pipe.unet.dtype)).latent_dist.sample()
+        def encode():
+            return pipe.vae.config.scaling_factor * pipe.vae.encode(imgs[lo:hi].to(pipe.unet.dtype)).latent_dist.sample()
+        # partners must hold the same latents: the posterior sample is drawn once, on the half-0 rank
+        latent_x0 = partner_share(layout, encode, (latents[lo:hi].shape, getattr(pipe.vae, "dtype", pipe.unet.dtype),
+                                                   latents.device)) if split else encode()
         latents_init = noise_scheduler.add_noise(latent_x0, latents[lo:hi], timesteps[num_warmup_steps]).detach()
     n_local = hi - lo
     chunks = 2 if do_classifier_free_guidance else 1
-    pe = chunk_frames(prompt_embeds, chunks, B, lo, hi)                       # (b f) layout: the frames of each chunk
+    if split:
+        layout.chunks(chunks)                                                   # the half layout needs both CFG halves
+    pe = prompt_embeds if layout is None else layout.rows(prompt_embeds, chunks)    # (b f) layout: the frames held
+    gather = layout_group(layout)                                               # record_latents: within the half
     sub_flows = sub_occs = sub_sal = None
     latents = latents_init
     for i, t in enumerate(timesteps[num_warmup_steps:]):
@@ -122,12 +149,13 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
             for f in range(2):
                 if lo <= f < hi:
                     latents[f - lo] = rec[f]
-            record_latents[i] = _gather_first_last(latents, B, lo, hi, shard)
+            record_latents[i] = _gather_first_last(latents, B, lo, hi, gather)
         else:
-            record_latents += [_gather_first_last(latents, B, lo, hi, shard)]
-        latent_model_input = torch.cat([latents] * 2) if do_classifier_free_guidance else latents
+            record_latents += [_gather_first_last(latents, B, lo, hi, gather)]
+        # one CFG half per rank in the half layout: its latents, prompt and edge rows only
+        latent_model_input = torch.cat([latents] * 2) if do_classifier_free_guidance and not split else latents
         if use_controlnet:
-            e = chunk_frames(edges, chunks, B, lo, hi)
+            e = edges if layout is None else layout.rows(edges, chunks)
             down_block_res_samples, mid_block_res_sample = controlnet(
                 latent_model_input, t, encoder_hidden_states=pe, controlnet_cond=e,
                 conditioning_scale=cond_scale[i + num_warmup_steps], guess_mode=False, return_dict=False)
@@ -143,5 +171,6 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
         smooth = (i + num_warmup_steps) in bg_smoothing_steps
         latents = step(pipe, noise_pred, t, latents, generator, visualize_pipeline=visualize_pipeline,
                        flows=flows if smooth else None, occs=occs if smooth else None, saliency=saliency if smooth else None,
-                       guidance_scale=guidance_scale if do_classifier_free_guidance else None, noise=noise, shard=shard)[0]
+                       guidance_scale=guidance_scale if do_classifier_free_guidance else None, noise=noise,
+                       shard=layout if split else shard)[0]
     return latents
