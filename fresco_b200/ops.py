@@ -166,10 +166,10 @@ def temporal_attn_fwd(q_raw, k_raw, v_src, fwd_map, traj_mask, chunks: int, head
     return out
 
 
-def _check_warp_operands(what, specs):
-    """Refuse, before any launch, operands the warp kernels would misread: the C ABI takes raw pointers, so a wrong
-    dtype, shape or layout would be read as something else or out of bounds.  specs: (name, tensor, dtype, allowed
-    shapes); dtypes, shapes and layouts are checked first, then that every operand is a CUDA tensor on one device."""
+def _check_operands(what, specs):
+    """Refuse, before any launch, operands a kernel would misread: the C ABI takes raw pointers, so a wrong dtype,
+    shape or layout would be read as something else or out of bounds.  specs: (name, tensor, dtype, allowed shapes);
+    dtypes, shapes and layouts are checked first, then that every operand is a CUDA tensor on one device."""
     for name, t, dtype, shapes in specs:
         if not isinstance(t, torch.Tensor):
             raise L.FrescoError(f"{what}: {name} must be a tensor")
@@ -192,7 +192,7 @@ def flow_warp(src: torch.Tensor, flow: torch.Tensor) -> torch.Tensor:
         raise L.FrescoError("flow_warp: src must be fp32 [B, C, h, w]")
     B, C, h, w = src.shape
     Bf = flow.shape[0] if isinstance(flow, torch.Tensor) and flow.dim() == 4 and flow.shape[0] > 0 else 1
-    _check_warp_operands("flow_warp", [("src", src, torch.float32, [src.shape]),
+    _check_operands("flow_warp", [("src", src, torch.float32, [src.shape]),
                                        ("flow", flow, torch.float32, [(Bf, 2, h, w)])])
     dst = torch.empty_like(src)
     L.check(L.lib().fresco_flow_warp(L.ptr(src), L.ptr(flow), L.ptr(dst), B, C, h, w, Bf, L.stream()),
@@ -216,7 +216,7 @@ def warp_fuse_chain(sample, bwd_flow, fwd_flow_last, blend, chunks: int, out=Non
              ("blend", blend, torch.float32, [(n, h, w), (n, 1, h, w)])]
     if out is not None:
         specs.append(("out", out, sample.dtype, [sample.shape]))
-    _check_warp_operands("warp_fuse_chain", specs)
+    _check_operands("warp_fuse_chain", specs)
     if out is None:
         out = torch.empty_like(sample)
     is_half = 1 if sample.dtype == torch.float16 else 0
@@ -419,6 +419,13 @@ def gram_grad(tsign, xhat, norms, grad_bcl, weight: float):
 
 
 def adam_step(param, grad, exp_avg, exp_avg_sq, step: int, lr=0.2, beta1=0.9, beta2=0.999, eps=1e-8):
+    """One torch.optim.Adam step in place on fp32 param, exp_avg, exp_avg_sq (all shaped like param) from grad."""
+    if not isinstance(param, torch.Tensor):
+        raise L.FrescoError("adam_step: param must be a tensor")
+    shape = [param.shape]
+    _check_operands("adam_step", [("param", param, torch.float32, shape), ("grad", grad, torch.float32, shape),
+                                  ("exp_avg", exp_avg, torch.float32, shape),
+                                  ("exp_avg_sq", exp_avg_sq, torch.float32, shape)])
     ev = _prof_begin()
     L.check(L.lib().fresco_adam_step(L.ptr(param), L.ptr(grad), L.ptr(exp_avg), L.ptr(exp_avg_sq), param.numel(),
                                      int(step), lr, beta1, beta2, eps, L.stream()), "fresco_adam_step")
@@ -426,11 +433,18 @@ def adam_step(param, grad, exp_avg, exp_avg_sq, step: int, lr=0.2, beta1=0.9, be
 
 
 def adain(content_f32: torch.Tensor, style: torch.Tensor) -> torch.Tensor:
+    """content fp32 and style fp16 / fp32, both [n, c, h, w] with h * w >= 2 -> out like style."""
+    if not isinstance(style, torch.Tensor) or style.dim() != 4:
+        raise L.FrescoError("adain: style must be [n, c, h, w]")
+    if style.dtype not in (torch.float16, torch.float32):
+        raise L.FrescoError("adain: fp16 or fp32 style only")
     n, c, h, w = style.shape
+    if h * w < 2:
+        raise L.FrescoError(f"adain: planes of {h * w} element(s) have no unbiased variance")
+    _check_operands("adain", [("style", style, style.dtype, [style.shape]),
+                              ("content", content_f32, torch.float32, [style.shape])])
     out = torch.empty_like(style)
     is_half = 1 if style.dtype == torch.float16 else 0
-    if not is_half and style.dtype != torch.float32:
-        raise L.FrescoError("adain: fp16 or fp32 style only")
     ev = _prof_begin()
     L.check(L.lib().fresco_adain(L.ptr(content_f32), L.ptr(style), L.ptr(out), is_half, n * c, h * w, L.stream()),
             "fresco_adain")
@@ -464,6 +478,11 @@ def gmflow_flow_attention(q: torch.Tensor, k: torch.Tensor, values: torch.Tensor
 
 def dilate(x: torch.Tensor, k: int) -> torch.Tensor:
     """fp32 [..., h, w] masks -> k x k dilation with replicate padding (src/utils.py:81-93)."""
+    if not isinstance(x, torch.Tensor) or x.dim() < 2 or x.numel() == 0:
+        raise L.FrescoError("dilate: x must be fp32 [..., h, w] with at least one element")
+    if not isinstance(k, int) or k <= 0 or k % 2 == 0:
+        raise L.FrescoError(f"dilate: the kernel size must be a positive odd int, got {k!r}")
+    _check_operands("dilate", [("x", x, torch.float32, [x.shape])])
     h, w = x.shape[-2], x.shape[-1]
     out = torch.empty_like(x)
     L.check(L.lib().fresco_dilate(L.ptr(x), L.ptr(out), x.numel() // (h * w), h, w, int(k), L.stream()), "fresco_dilate")
@@ -473,6 +492,13 @@ def dilate(x: torch.Tensor, k: int) -> torch.Tensor:
 def cfg_pred_x0(noise_pred_2n: torch.Tensor, sample: torch.Tensor, guidance_scale: float, alpha_prod_t: float,
                 do_cfg: bool = True) -> torch.Tensor:
     """noise_pred [2N, ...] (uncond | text chunks, or [N, ...] when do_cfg is False), sample [N, ...] -> predicted x0."""
+    if not isinstance(sample, torch.Tensor) or sample.dim() < 1 or sample.numel() == 0:
+        raise L.FrescoError("cfg_pred_x0: sample must be a non-empty [N, ...] tensor")
+    if sample.dtype not in (torch.float16, torch.float32):
+        raise L.FrescoError("cfg_pred_x0: fp16 or fp32 only")
+    halves = (2 * sample.shape[0],) if do_cfg else (sample.shape[0],)
+    _check_operands("cfg_pred_x0", [("sample", sample, sample.dtype, [sample.shape]),
+                                    ("noise_pred", noise_pred_2n, sample.dtype, [halves + tuple(sample.shape[1:])])])
     n = sample.numel()
     x0 = torch.empty_like(sample)
     is_half = 1 if sample.dtype == torch.float16 else 0
@@ -484,6 +510,16 @@ def cfg_pred_x0(noise_pred_2n: torch.Tensor, sample: torch.Tensor, guidance_scal
 
 
 def ddpm_prev(x0, sample, noise, c_x0: float, c_xt: float, sigma: float, repeat_noise: bool = False):
+    """x0, sample [N, ...]; noise like sample, or (repeat_noise) [1, ...] or like sample with frame 0 used for every
+    frame -> the previous sample."""
+    if not isinstance(sample, torch.Tensor) or sample.dim() < 1 or sample.numel() == 0:
+        raise L.FrescoError("ddpm_prev: sample must be a non-empty [N, ...] tensor")
+    if sample.dtype not in (torch.float16, torch.float32):
+        raise L.FrescoError("ddpm_prev: fp16 or fp32 only")
+    noise_shapes = [sample.shape] + ([(1,) + tuple(sample.shape[1:])] if repeat_noise else [])
+    _check_operands("ddpm_prev", [("sample", sample, sample.dtype, [sample.shape]),
+                                  ("x0", x0, sample.dtype, [sample.shape]),
+                                  ("noise", noise, sample.dtype, noise_shapes)])
     prev = torch.empty_like(sample)
     is_half = 1 if sample.dtype == torch.float16 else 0
     per_frame = sample[0].numel()

@@ -84,6 +84,62 @@ def test_warp_operand_errors_do_not_touch_the_gpu():
         ops.flow_warp(src, torch.zeros(2, 2, h, w))
 
 
+def test_step_operand_errors_do_not_touch_the_gpu():
+    """ops.adam_step, adain, cfg_pred_x0, ddpm_prev and dilate check every operand's dtype, shape and layout before the
+    device, so each mistake is refused with its own message (never read through a raw pointer), here on CPU tensors."""
+    from fresco_b200 import ops
+    from fresco_b200._lib import FrescoError
+    z = torch.zeros
+    n = 40
+    adam = {"param": z(n), "grad": z(n), "exp_avg": z(n), "exp_avg_sq": z(n)}
+    for name, t, msg in (("grad", z(n - 1), "grad must have shape"), ("grad", z(n, dtype=torch.float16),
+                                                                      "grad must be torch.float32"),
+                         ("param", z(n, dtype=torch.float64), "param must be torch.float32"),
+                         ("exp_avg", z(n, 2)[:, 0], "exp_avg must be contiguous"),
+                         ("exp_avg_sq", z(2 * n), "exp_avg_sq must have shape")):
+        a = dict(adam, **{name: t})
+        with pytest.raises(FrescoError, match=msg):
+            ops.adam_step(a["param"], a["grad"], a["exp_avg"], a["exp_avg_sq"], 1)
+    with pytest.raises(FrescoError, match="param must be a CUDA tensor"):
+        ops.adam_step(*adam.values(), 1)
+    style = z(2, 3, 4, 5, dtype=torch.float16)
+    for content, sty, msg in ((z(2, 3, 4, 5, dtype=torch.float16), style, "content must be torch.float32"),
+                              (z(2, 3, 20), style, "content must have shape"),
+                              (z(2, 3, 5, 4).transpose(2, 3), style, "content must be contiguous"),
+                              (z(2, 3, 4, 5), z(2, 3, 20), "style must be"),
+                              (z(2, 3, 4, 5), z(2, 3, 4, 5, dtype=torch.float64), "fp16 or fp32 style"),
+                              (z(2, 3, 1, 1), z(2, 3, 1, 1), "no unbiased variance"),
+                              (z(2, 3, 4, 5), style, "style must be a CUDA tensor")):
+        with pytest.raises(FrescoError, match=msg):
+            ops.adain(content, sty)
+    N, shp = 3, (4, 6, 5)
+    sample, pred = z(N, *shp), z(2 * N, *shp)
+    for args, kw, msg in (((z(N, *shp), sample, 7.5, 0.5), {}, "noise_pred must have shape"),
+                          ((pred, sample, 7.5, 0.5), {"do_cfg": False}, "noise_pred must have shape"),
+                          ((pred.half(), sample, 7.5, 0.5), {}, "noise_pred must be torch.float32"),
+                          ((pred, sample.double(), 7.5, 0.5), {}, "fp16 or fp32"),
+                          ((z(2 * N, 6, 4, 5), sample, 7.5, 0.5), {}, "noise_pred must have shape"),
+                          ((pred, sample, 7.5, 0.5), {}, "sample must be a CUDA tensor")):
+        with pytest.raises(FrescoError, match=msg):
+            ops.cfg_pred_x0(*args, **kw)
+    for x0, noise, rep, msg in ((z(N, *shp), z(1, *shp), False, "noise must have shape"),
+                                (z(N, *shp), z(N * 120), True, "noise must have shape"),
+                                (z(N - 1, *shp), z(N, *shp), False, "x0 must have shape"),
+                                (z(N, *shp).half(), z(N, *shp), False, "x0 must be torch.float32"),
+                                (z(N, *shp), z(N, *shp).half(), True, "noise must be torch.float32"),
+                                (z(N, *shp), z(1, *shp), True, "sample must be a CUDA tensor"),
+                                (z(N, *shp), z(N, *shp), True, "sample must be a CUDA tensor")):
+        with pytest.raises(FrescoError, match=msg):
+            ops.ddpm_prev(x0, sample, noise, 1.0, 0.5, 0.1, repeat_noise=rep)
+    for x, k, msg in ((z(2, 1, 8, 8), 4, "positive odd int"), (z(2, 1, 8, 8), 0, "positive odd int"),
+                      (z(2, 1, 8, 8), 5.0, "positive odd int"), (z(8), 5, "x must be fp32"),
+                      (z(2, 0, 8, 8), 5, "x must be fp32"), (z(2, 1, 8, 8, dtype=torch.float16), 5, "x must be torch.float32"),
+                      (z(2, 1, 8, 8).transpose(2, 3), 5, "x must be contiguous"),
+                      (z(2, 1, 8, 8), 5, "x must be a CUDA tensor")):
+        with pytest.raises(FrescoError, match=msg):
+            ops.dilate(x, k)
+
+
 def test_default_attention_kernel_per_head_dim(built_lib):
     """Host-side kernel selection through the C ABI (no launch): the default variant per head_dim, the options select
     the other parity-tested variants, negative values restore the defaults, unknown names fail."""

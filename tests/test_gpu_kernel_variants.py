@@ -518,17 +518,21 @@ COVERED_ELSEWHERE = {
                         "test_gpu_kernels.py::test_flow_warp_and_consistency)",
     "warp_taps_kernel": "test_gpu_warp_loss.py::test_warp_taps_bit_exact (and it builds the adjoint of every "
                         "temporal-loss row here)",
-    "adam_kernel": "test_gpu_kernels.py::test_adam_matches_torch",
-    "adain_kernel<half>": "test_gpu_kernels.py::test_adain_eps_quirk",
-    "adain_kernel<float>": "test_gpu_kernels.py::test_adain_eps_quirk",
-    "cfg_pred_x0_kernel<half>": "test_gpu_parity_r2.py::test_ddpm_step_kernels_and_dilate_golden",
-    "cfg_pred_x0_kernel<float>": "test_gpu_parity_r2.py::test_ddpm_step_kernels_and_dilate_golden",
-    "ddpm_prev_kernel<half>": "test_gpu_parity_r2.py::test_ddpm_step_kernels_and_dilate_golden",
-    "ddpm_prev_kernel<float>": "test_gpu_parity_r2.py::test_ddpm_step_kernels_and_dilate_golden",
-    "dilate_kernel": "test_gpu_parity_r2.py::test_ddpm_step_kernels_and_dilate_golden",
+    "adam_kernel": "test_gpu_step_kernels.py::test_adam_family (within oracle.step_bound; also test_adam_layer3_size)",
+    "adain_kernel<half>": "test_gpu_step_kernels.py::test_adain_family (within oracle.step_bound; also "
+                          "test_adain_decoder_layers)",
+    "adain_kernel<float>": "test_gpu_step_kernels.py::test_adain_family (within oracle.step_bound; also "
+                           "test_adain_decoder_layers)",
+    "cfg_pred_x0_kernel<half>": "test_gpu_step_kernels.py::test_cfg_and_ddpm_family (within oracle.step_bound)",
+    "cfg_pred_x0_kernel<float>": "test_gpu_step_kernels.py::test_cfg_and_ddpm_family (within oracle.step_bound)",
+    "ddpm_prev_kernel<half>": "test_gpu_step_kernels.py::test_cfg_and_ddpm_family (within oracle.step_bound)",
+    "ddpm_prev_kernel<float>": "test_gpu_step_kernels.py::test_cfg_and_ddpm_family (within oracle.step_bound)",
+    "dilate_kernel": "test_gpu_step_kernels.py::test_dilate_family (within oracle.step_bound; binary and dyadic "
+                     "bit-exact)",
     "to_token_major_f16_kernel": "test_gpu_gmflow.py::test_corr_families (the first two launches of every call; the "
                                  "fp16 rounding it does is what gmflow_bound evaluates)",
-    "mapping_single_kernel": "test_gpu_kernels.py::test_mapping_bit_exact_golden",
+    "mapping_single_kernel": "test_mapping_conflicts.py::test_kernel_equals_the_oracle (bit-exact; also "
+                             "test_gpu_kernels.py::test_mapping_bit_exact_golden)",
 }
 
 
