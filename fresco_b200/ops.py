@@ -366,6 +366,9 @@ def warp_loss_fwd_bwd(cs, fwd_flow, bwd_flow, fwd_keep, bwd_keep, grad, loss_acc
 
 def gram_normalize(cs_bcl: torch.Tensor):
     """cs [B, C, L] fp32 -> xhat [B, L, C] fp16, norms [B, L] fp32."""
+    if not isinstance(cs_bcl, torch.Tensor) or cs_bcl.dim() != 3:
+        raise L.FrescoError("gram_normalize: cs must be fp32 [B, C, L]")
+    _check_operands("gram_normalize", [("cs", cs_bcl, torch.float32, [cs_bcl.shape])])
     B, C, Lt = cs_bcl.shape
     xhat = torch.empty(B, Lt, C, dtype=torch.float16, device=cs_bcl.device)
     norms = torch.empty(B, Lt, dtype=torch.float32, device=cs_bcl.device)
@@ -382,8 +385,20 @@ def _gram_scale(weight: float, B: int, Lt: int) -> float:
     return float(weight) / (B * Lt * Lt)
 
 
+def _gram_shape(what, xhat):
+    if not isinstance(xhat, torch.Tensor) or xhat.dim() != 3:
+        raise L.FrescoError(f"{what}: xhat must be fp16 [B, L, C]")
+    return xhat.shape
+
+
+def _loss_spec(loss_acc):
+    return [] if loss_acc is None else [("loss_acc", loss_acc, torch.float32, [(1,), ()])]
+
+
 def gram_sign(xhat, target, weight: float, loss_acc=None):
-    B, Lt, C = xhat.shape
+    B, Lt, C = _gram_shape("gram_sign", xhat)
+    _check_operands("gram_sign", [("xhat", xhat, torch.float16, [(B, Lt, C)]),
+                                  ("target", target, torch.float32, [(B, Lt, Lt)])] + _loss_spec(loss_acc))
     tsign = torch.empty(B, Lt, Lt, dtype=torch.float16, device=xhat.device)
     ev = _prof_begin()
     L.check(L.lib().fresco_gram_sign_scaled(L.ptr(xhat), L.ptr(target), L.ptr(tsign),
@@ -396,7 +411,9 @@ def gram_sign(xhat, target, weight: float, loss_acc=None):
 def gram_sign_ref(xhat, yhat, weight: float, loss_acc=None):
     """T = 2 sign(xhat xhat^T - yhat yhat^T) with the target recomputed in the kernel from the normalised reference
     features yhat [B, L, C] fp16 (no [B, L, L] fp32 target)."""
-    B, Lt, C = xhat.shape
+    B, Lt, C = _gram_shape("gram_sign_ref", xhat)
+    _check_operands("gram_sign_ref", [("xhat", xhat, torch.float16, [(B, Lt, C)]),
+                                      ("yhat", yhat, torch.float16, [(B, Lt, C)])] + _loss_spec(loss_acc))
     tsign = torch.empty(B, Lt, Lt, dtype=torch.float16, device=xhat.device)
     ev = _prof_begin()
     L.check(L.lib().fresco_gram_sign_ref_scaled(L.ptr(xhat), L.ptr(yhat), L.ptr(tsign),
@@ -407,7 +424,11 @@ def gram_sign_ref(xhat, yhat, weight: float, loss_acc=None):
 
 
 def gram_grad(tsign, xhat, norms, grad_bcl, weight: float):
-    B, Lt, C = xhat.shape
+    B, Lt, C = _gram_shape("gram_grad", xhat)
+    _check_operands("gram_grad", [("xhat", xhat, torch.float16, [(B, Lt, C)]),
+                                  ("tsign", tsign, torch.float16, [(B, Lt, Lt)]),
+                                  ("norms", norms, torch.float32, [(B, Lt)]),
+                                  ("grad", grad_bcl, torch.float32, [(B, C, Lt)])])
     nbytes = int(L.lib().fresco_gram_grad_workspace_bytes(B, Lt, C))
     ws = _workspace(("gram_grad", xhat.device), max(nbytes, 16), xhat.device)
     ev = _prof_begin()

@@ -84,6 +84,40 @@ def test_warp_operand_errors_do_not_touch_the_gpu():
         ops.flow_warp(src, torch.zeros(2, 2, h, w))
 
 
+def test_gram_operand_errors_do_not_touch_the_gpu():
+    """ops.gram_normalize, gram_sign, gram_sign_ref and gram_grad check every operand's dtype, shape and layout before
+    the device, so each mistake is refused with its own message (never read through a raw pointer), here on CPU
+    tensors."""
+    from fresco_b200 import ops
+    from fresco_b200._lib import FrescoError
+    z = torch.zeros
+    B, L, C = 2, 5, 16
+    for cs, msg in ((z(B, C, L, dtype=torch.float16), "cs must be torch.float32"), (z(B, C * L), "cs must be fp32"),
+                    (z(B, L, C).transpose(1, 2), "cs must be contiguous"), (z(B, C, L), "cs must be a CUDA tensor")):
+        with pytest.raises(FrescoError, match=msg):
+            ops.gram_normalize(cs)
+    xh, tgt = z(B, L, C, dtype=torch.float16), z(B, L, L)
+    for x, t, loss, msg in ((xh.float(), tgt, None, "xhat must be torch.float16"), (xh[0], tgt, None, "xhat must be fp16"),
+                            (xh, z(B, L, L + 1), None, "target must have shape"),
+                            (xh, tgt.half(), None, "target must be torch.float32"),
+                            (xh, tgt.transpose(1, 2), None, "target must be contiguous"),
+                            (xh, tgt, z(2), "loss_acc must have shape"), (xh, tgt, None, "xhat must be a CUDA tensor")):
+        with pytest.raises(FrescoError, match=msg):
+            ops.gram_sign(x, t, 100.0, loss)
+    for y, msg in ((z(B, L, C), "yhat must be torch.float16"), (z(B, L + 1, C, dtype=torch.float16), "yhat must have"),
+                   (xh, "xhat must be a CUDA tensor")):
+        with pytest.raises(FrescoError, match=msg):
+            ops.gram_sign_ref(xh, y, 100.0)
+    ts, nr, gr = z(B, L, L, dtype=torch.float16), z(B, L), z(B, C, L)
+    for args, msg in (((ts.float(), xh, nr, gr), "tsign must be torch.float16"),
+                      ((ts, xh, z(B, L + 1), gr), "norms must have shape"),
+                      ((ts, xh, nr, z(B, L, C)), "grad must have shape"),
+                      ((ts, xh, nr, z(B, L, C).transpose(1, 2)), "grad must be contiguous"),
+                      ((ts, xh, nr, gr), "xhat must be a CUDA tensor")):
+        with pytest.raises(FrescoError, match=msg):
+            ops.gram_grad(*args, 100.0)
+
+
 def test_step_operand_errors_do_not_touch_the_gpu():
     """ops.adam_step, adain, cfg_pred_x0, ddpm_prev and dilate check every operand's dtype, shape and layout before the
     device, so each mistake is refused with its own message (never read through a raw pointer), here on CPU tensors."""

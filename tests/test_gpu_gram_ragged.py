@@ -9,7 +9,7 @@ stride that is not a multiple of 16 bytes, so the launchers pick the ragged inst
 * padding invariance: zero-padding X^, Y^ and the dense target to roundup(L, 8) and running the aligned call gives the
   same T, g^ and gradient bit for bit, and the same loss up to the order of the cross-CTA sum, on every entry point,
   both products FRESCO_GRAM_V selects and the _scaled forms;
-* every output against fp64 with the criteria of the gram rows of test_gpu_kernel_variants.py;
+* every output against fp64 within ``oracle.gram_bound`` (``tests/test_gpu_gram.py`` runs its input families);
 * NaN-prefilled outputs between NaN guard rows: every element written, no guard touched;
 * the launch names: the parent instantiations at aligned counts, the ragged ones otherwise;
 * optimize_feature at every failing (resolution, aspect ratio) setting against the CPU oracle, and one harness-UNet
@@ -25,6 +25,8 @@ import pytest
 import torch
 
 from oracle import fresco_oracle as O
+from oracle import gram_bound as GB
+from oracle.gram_bound import Run, launched
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "fresco_b200", "csrc")
@@ -97,27 +99,6 @@ def P(t):
     return t.data_ptr()
 
 
-GUARD = 8                                                            # guard rows before and after an output
-
-
-def guarded(B, R, W, dtype, fill=float("nan")):
-    """(buffer, view): a contiguous [B, R, W] view between GUARD NaN rows of W elements on each side, prefilled
-    with ``fill``."""
-    buf = torch.full((B * R + 2 * GUARD, W), float("nan"), dtype=dtype, device="cuda")
-    view = buf[GUARD:GUARD + B * R].view(B, R, W)
-    view.fill_(fill)
-    return buf, view
-
-
-def guards_intact(buf, what):
-    assert torch.isnan(buf[:GUARD]).all() and torch.isnan(buf[-GUARD:]).all(), f"{what}: a guard row was written"
-
-
-def launched(fb, what, rc, want):
-    fb.lib.check(rc, what)
-    assert fb.lib.last_kernel() == want, f"{what} launched {fb.lib.last_kernel()}, expected {want}"
-
-
 def same_bits(a, b, what):
     assert a.shape == b.shape, (what, a.shape, b.shape)
     ai = a.contiguous().view(torch.int16 if a.element_size() == 2 else torch.int32)
@@ -131,68 +112,6 @@ def atomic_tol(loss):
     8 * SMs additions rounds once."""
     n = 8 * torch.cuda.get_device_properties(0).multi_processor_count
     return n * 2.0 ** -24 * abs(loss) + 1e-30
-
-
-def names(L):
-    ragged = L % 8 != 0
-    return {"sign_ref": "gram2_kernel<G2_SIGN,ragged>" if ragged else "gram2_kernel<G2_SIGN>",
-            "tx": "gram2_kernel<G2_GRAD,ragged>" if ragged else "gram2_kernel<G2_GRAD>",
-            "sign": "tile_gemm_kernel<EPI_GRAM_SIGN,0>", "grad": "gram_project_kernel"}
-
-
-class Run:
-    """Every Gram entry point on one set of operands, outputs between NaN guard rows."""
-
-    def __init__(self, fb, xhat, yhat, norms, target, grad0, weight, scale, L_names):
-        self.fb = fb
-        B, L, C = xhat.shape
-        st = fb.lib.stream()
-        want = names(L_names)
-        self.t_buf, self.tsign = guarded(B, L, L, torch.float16)
-        self.loss = torch.zeros(1, device="cuda")
-        launched(fb, "fresco_gram_sign_ref_scaled", fb.c.fresco_gram_sign_ref_scaled(
-            P(xhat), P(yhat), P(self.tsign), P(self.loss), B, L, C, scale, st), want["sign_ref"])
-        self.t1_buf, self.tsign1 = guarded(B, L, L, torch.float16)
-        self.loss1 = torch.zeros(1, device="cuda")
-        launched(fb, "fresco_gram_sign_ref", fb.c.fresco_gram_sign_ref(
-            P(xhat), P(yhat), P(self.tsign1), P(self.loss1), B, L, C, weight, st), want["sign_ref"])
-        self.td_buf, self.tsign_d = guarded(B, L, L, torch.float16)
-        self.loss_d = torch.zeros(1, device="cuda")
-        launched(fb, "fresco_gram_sign_scaled", fb.c.fresco_gram_sign_scaled(
-            P(xhat), P(target), P(self.tsign_d), P(self.loss_d), B, L, C, scale, st), want["sign"])
-        self.g_buf, self.ghat = guarded(B, L, C, torch.float32)
-        launched(fb, "fresco_gram_tx", fb.c.fresco_gram_tx(P(self.tsign), P(xhat), P(self.ghat), B, L, C, scale, st),
-                 want["tx"])
-        nbytes = int(fb.c.fresco_gram_grad_workspace_bytes(B, L, C))
-        assert nbytes == B * L * C * 4
-        ws = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
-        self.grads, self.grad_bufs = {}, {}
-        try:
-            for v in (2, 1):
-                fb.lib.set_option("FRESCO_GRAM_V", v)
-                for form in ("scaled", "weight"):
-                    gb, gr = guarded(B, C, L, torch.float32)
-                    gr.copy_(grad0)
-                    if form == "scaled":
-                        rc = fb.c.fresco_gram_grad_scaled(P(self.tsign), P(xhat), P(norms), P(gr), B, L, C, scale, P(ws),
-                                                          nbytes, st)
-                    else:
-                        rc = fb.c.fresco_gram_grad(P(self.tsign), P(xhat), P(norms), P(gr), B, L, C, weight, P(ws),
-                                                   nbytes, st)
-                    launched(fb, f"fresco_gram_grad_{form} (FRESCO_GRAM_V={v})", rc, want["grad"])
-                    self.grads[(v, form)], self.grad_bufs[(v, form)] = gr, gb
-        finally:
-            fb.lib.set_option("FRESCO_GRAM_V", -1)
-        torch.cuda.synchronize()
-
-    def hygiene(self):
-        for what, buf, out in (("T (scaled)", self.t_buf, self.tsign), ("T", self.t1_buf, self.tsign1),
-                               ("T (dense target)", self.td_buf, self.tsign_d), ("g^", self.g_buf, self.ghat)):
-            guards_intact(buf, what)
-            assert torch.isfinite(out).all(), f"{what}: {(~torch.isfinite(out)).sum().item()} elements not written"
-        for key, buf in self.grad_bufs.items():
-            guards_intact(buf, f"grad {key}")
-            assert torch.isfinite(self.grads[key]).all(), f"grad {key} not finite"
 
 
 def operands(B, L, C, seed):
@@ -212,11 +131,7 @@ def normalize(fb, src):
     norms = torch.full((B, L), float("nan"), dtype=torch.float32, device="cuda")
     launched(fb, "fresco_gram_normalize", fb.c.fresco_gram_normalize(P(src), P(xhat), P(norms), B, C, L,
                                                                      fb.lib.stream()), "gram_normalize_kernel")
-    n64 = src.double().norm(dim=1)
-    assert (norms.double() - n64).abs().max().item() <= C * 2.0 ** -23 * n64.max().item()
-    x64 = (src.double() / n64[:, None]).transpose(1, 2)
-    err = (xhat.double() - x64).abs()
-    assert torch.isfinite(xhat).all() and (err <= (2.0 ** -11 + C * 2.0 ** -23) * x64.abs() + 2.0 ** -25).all()
+    GB.check_normalize(src, xhat, norms)
     return xhat, norms
 
 
@@ -227,58 +142,6 @@ def pad_tokens(t, Lp, dims):
         shape[d] = Lp - t.shape[d]
         t = torch.cat([t, torch.zeros(shape, dtype=t.dtype, device=t.device)], d)
     return t.contiguous()
-
-
-def check_fp64(run, xhat, yhat, norms, target, grad0, weight):
-    """test_gpu_kernel_variants.py's gram criteria.  The one addition: a diagonal entry D_ii = |x^_i|^2 - |y^_i|^2 is
-    itself at rounding level, so the loss gets the band for each of the B * L diagonal entries on top of 1e-4 relative
-    (it matters only at the smallest token counts, where the diagonal is a large share of the entries)."""
-    B, L, C = xhat.shape
-    alpha = weight / (B * L * L)
-    band = 2 * C * 2.0 ** -22
-    loss_ref, in_band = 0.0, 0
-    offdiag = ~torch.eye(L, dtype=torch.bool, device="cuda")
-    for b in range(B):
-        X, Y = xhat[b].double(), yhat[b].double()
-        D = X @ X.T - Y @ Y.T
-        t = run.tsign[b].double()
-        assert ((t == 2) | (t == 0) | (t == -2)).all(), f"batch {b}: tsign entries not in {{-2, 0, 2}}"
-        outside = D.abs() > band
-        bad = (t != 2 * torch.sign(D)) & outside
-        assert not bad.any(), f"batch {b}: {bad.sum().item()} signs wrong"
-        loss_ref += D.abs().sum().item()
-        in_band += ((~outside) & offdiag).sum().item()
-    assert in_band <= 0.05 * B * L * (L - 1), f"{in_band} off-diagonal entries inside the accumulation band"
-    loss_ref *= alpha
-    tol = 1e-4 * loss_ref + alpha * B * L * band
-    assert abs(run.loss.item() - loss_ref) <= tol, (run.loss.item(), loss_ref, tol)
-    for b in range(B):
-        T, X = run.tsign[b].double(), xhat[b].double()
-        g64 = alpha * (T @ X)
-        e = 2.0 ** -20 * math.sqrt(L) * alpha * (T.abs() @ X.abs()) + 2.0 ** -22 * g64.abs()
-        ratio = (run.ghat[b].double() - g64).abs() / e
-        assert not (ratio > 1).any(), f"gram_tx batch {b}: worst err/tol {ratio.nan_to_num(nan=float('inf')).max():.3g}"
-        dot = (g64 * X).sum(1, keepdim=True)
-        nrm = norms[b].double()[:, None]
-        proj = (g64 - dot * X) / nrm
-        dot_err = (e * X.abs()).sum(1, keepdim=True) + C * 2.0 ** -23 * (g64 * X).abs().sum(1, keepdim=True)
-        tol = (e + X.abs() * dot_err + 2.0 ** -22 * (g64.abs() + (dot * X).abs())) / nrm
-        want = grad0[b].double().T + proj
-        tol = tol + 2.0 ** -23 * want.abs()
-        for key, gr in run.grads.items():
-            ratio = (gr[b].double().T - want).abs() / tol
-            assert not (ratio > 1).any(), f"gram_grad {key} batch {b}: worst err/tol {ratio.max():.3g}"
-    # the dense target: T = sign(G - A) + sign(G - A^T), loss over |G - A|
-    band2, ref2 = C * 2.0 ** -22, 0.0
-    for b in range(B):
-        G = xhat[b].double() @ xhat[b].double().T
-        d1, d2 = G - target[b].double(), G - target[b].double().T
-        t = run.tsign_d[b].double()
-        bad = (t != torch.sign(d1) + torch.sign(d2)) & (d1.abs() > band2) & (d2.abs() > band2)
-        assert not bad.any(), f"dense target batch {b}: {bad.sum().item()} signs wrong"
-        ref2 += d1.abs().sum().item()
-    ref2 *= alpha
-    assert abs(run.loss_d.item() - ref2) <= 1e-4 * ref2 + alpha * B * L * band2, (run.loss_d.item(), ref2)
 
 
 # ------------------------------------------------------------------------------------------------ the kernels
@@ -297,14 +160,14 @@ def test_gram_entry_points(fb, L, C, N):
     for b in range(B):
         target[b] = (xhat[b].double() @ xhat[b].double().T
                      + 0.05 * torch.randn(L, L, device="cuda", generator=g, dtype=torch.float64)).float()
-    run = Run(fb, xhat, yhat, norms, target, grad0, weight, scale, L)
+    run = Run(fb, xhat, yhat, norms, target, grad0, weight, scale)
     run.hygiene()
     # the weight form divides in double and rounds once: the same fp32 scale, so the same bits
     same_bits(run.tsign1, run.tsign, "T (weight form)")
     assert abs(run.loss1.item() - run.loss.item()) <= atomic_tol(run.loss.item())
     for v in (2, 1):
         same_bits(run.grads[(v, "weight")], run.grads[(v, "scaled")], f"grad V={v} (weight form)")
-    check_fp64(run, xhat, yhat, norms, target, grad0, weight)
+    GB.check_run(run, xhat, yhat, norms, target, grad0, scale, torch.cuda.get_device_properties(0).multi_processor_count)
     if Lp == L:
         return
     # padding invariance: the aligned instantiations on operands zero-padded to Lp, with the same fp32 scale
@@ -422,12 +285,14 @@ def test_optimize_feature_teacher_forced(fb, hw, layer):
     assert cos >= 0.999, cos
     xhat, _ = fb.ops.gram_normalize(cs.reshape(B, C, L).cuda())
     tsign = fb.ops.gram_sign_ref(xhat, target.yhat, 100.0)
-    D = torch.stack([xhat[b].double() @ xhat[b].double().T - target.yhat[b].double() @ target.yhat[b].double().T
-                     for b in range(B)])
-    outside = D.abs() > 2 * C * 2.0 ** -22
-    loss16 = ref_trace[0]["temporal"] + 100.0 / (B * L * L) * D.abs().sum().item()
+    abs_sum = 0.0
+    for b in range(B):
+        D, beta = GB.sign_ref_band(xhat[b], target.yhat[b])
+        n, r = GB.sign_ref_check(tsign[b], D, beta)
+        assert n == 0, f"batch {b}: {n} signs wrong outside the band (worst |D|/beta {r:.3g})"
+        abs_sum += D.abs().sum().item()
+    loss16 = ref_trace[0]["temporal"] + 100.0 / (B * L * L) * abs_sum
     assert abs(tr.losses[0] - loss16) <= 1e-4 * loss16, (tr.losses[0], loss16)
-    assert torch.equal(tsign.double()[outside], 2 * torch.sign(D)[outside])
 
 
 @pytest.mark.gpu

@@ -32,6 +32,7 @@ import torch.nn.functional as F
 from oracle import attention_bound as AB
 from oracle import fresco_oracle as O
 from oracle import gmflow_bound as GB
+from oracle import gram_bound as GRB
 from oracle import temporal_bound as TB
 from oracle import warp_chain_bound as CB
 from oracle import warp_loss_bound as WB
@@ -398,8 +399,9 @@ row("gmflow-flow-attention-16x4096x128", ["tile_gemm_kernel<EPI_GMFLOW,0>"], _gm
 
 # ================================================================================================ Gram loss
 def _gram(fb, launch, B, C, h, w, dense=False, weight=100.0, seed=0):
-    """The spatial-consistency loss at a layer shape, operand-exact: every fp64 reference is computed from the kernels'
-    own fp16 xhat / yhat / tsign, one batch at a time on the GPU."""
+    """The spatial-consistency loss at a layer shape, operand-exact and elementwise within ``oracle.gram_bound``
+    (``tests/test_gpu_gram.py`` runs its input families): every fp64 reference is computed from the kernels' own fp16
+    xhat / yhat / tsign, one batch at a time on the GPU."""
     L = h * w
     g = torch.Generator(device="cuda").manual_seed(seed + C + L)
     base = torch.randn(B, C, 1, device="cuda", generator=g)
@@ -411,91 +413,49 @@ def _gram(fb, launch, B, C, h, w, dense=False, weight=100.0, seed=0):
     for src in (cs, cs_ref):
         xhat, norms = _nan((B, L, C), torch.float16), _nan((B, L), torch.float32)
         launch("fresco_gram_normalize", fb.c.fresco_gram_normalize(P(src), P(xhat), P(norms), B, C, L, st))
-        n64 = src.double().norm(dim=1)
-        _check_close(norms, n64, C * 2.0 ** -23 * n64.max().item(), "gram norms")
-        x64 = (src.double() / n64[:, None]).transpose(1, 2)
-        err = (xhat.double() - x64).abs()
-        assert torch.isfinite(xhat).all() and (err <= (2.0 ** -11 + C * 2.0 ** -23) * x64.abs() + 2.0 ** -25).all()
+        GRB.check_normalize(src, xhat, norms)
         normed.append((xhat, norms))
     (xhat, norms), (yhat, _) = normed
-    # ---- sign matrix with the recomputed target: D = X X^T - Y Y^T in one K = 2C contraction of exact fp16 products,
-    #      fp32 accumulation: |D_kernel - D| <= 2C * 2^-23 * sum|terms| <= 2C * 2^-22 (rows of unit norm)
-    tsign = _nan((B, L, L), torch.float16)
-    loss = torch.zeros(1, device="cuda")
-    launch("fresco_gram_sign_ref", fb.c.fresco_gram_sign_ref(P(xhat), P(yhat), P(tsign), P(loss), B, L, C, weight, st))
-    band = 2 * C * 2.0 ** -22
-    loss_ref, in_band = 0.0, 0
-    for b in range(B):
-        X, Y = xhat[b].double(), yhat[b].double()
-        D = X @ X.T - Y @ Y.T
-        t = tsign[b].double()
-        assert ((t == 2) | (t == 0) | (t == -2)).all(), f"batch {b}: tsign entries not in {{-2, 0, 2}} (unwritten: NaN)"
-        outside = D.abs() > band
-        bad = (t != 2 * torch.sign(D)) & outside
-        assert not bad.any(), f"batch {b}: {bad.sum().item()} signs wrong; " + _worst_tile(bad.double() * 2)
-        loss_ref += D.abs().sum().item()
-        in_band += (~outside).sum().item()
-        del D, t, bad, outside
-    assert in_band < 0.05 * B * L * L, f"{in_band} of {B * L * L} entries inside the accumulation band"
-    loss_ref *= weight / (B * L * L)
-    assert abs(loss.item() - loss_ref) < 1e-4 * loss_ref, (loss.item(), loss_ref)
+    scale = weight / (B * L * L)
+
+    class Out:
+        pass
+    run = Out()
+    run.t1_buf, run.td_buf = True, None
+    # ---- sign matrix with the recomputed target: D = X X^T - Y Y^T in one K = 2C contraction
+    run.tsign = _nan((B, L, L), torch.float16)
+    run.loss = torch.zeros(1, device="cuda")
+    launch("fresco_gram_sign_ref", fb.c.fresco_gram_sign_ref(P(xhat), P(yhat), P(run.tsign), P(run.loss), B, L, C,
+                                                             weight, st))
     # ---- ghat = alpha T X (tensor-core product of the backward), from the kernel's own T
-    alpha = weight / (B * L * L)
-    ghat = _nan((B, L, C), torch.float32)
-    launch("fresco_gram_tx", fb.c.fresco_gram_tx(P(tsign), P(xhat), P(ghat), B, L, C, alpha, st))
+    run.ghat = _nan((B, L, C), torch.float32)
+    launch("fresco_gram_tx", fb.c.fresco_gram_tx(P(run.tsign), P(xhat), P(run.ghat), B, L, C, scale, st))
     # ---- grad += projection of ghat through the normalisation Jacobian, under both products fresco_gram_grad can use
     grad0 = torch.zeros(B, C, L, device="cuda")
     nbytes = int(fb.c.fresco_gram_grad_workspace_bytes(B, L, C))
     ws = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
-    grads = {}
+    run.grads = {}
     for v in (2, 1):
         fb.lib.set_option("FRESCO_GRAM_V", v)
         gr = grad0.clone()
         launch(f"fresco_gram_grad (FRESCO_GRAM_V={v})",
-               fb.c.fresco_gram_grad(P(tsign), P(xhat), P(norms), P(gr), B, L, C, weight, P(ws), nbytes, st))
-        grads[v] = gr
+               fb.c.fresco_gram_grad(P(run.tsign), P(xhat), P(norms), P(gr), B, L, C, weight, P(ws), nbytes, st))
+        run.grads[v] = gr
     fb.lib.set_option("FRESCO_GRAM_V", -1)
-    for b in range(B):
-        T, X = tsign[b].double(), xhat[b].double()
-        g64 = alpha * (T @ X)
-        # fp32 accumulation over L terms: sqrt(L) 2^-20 of sum|terms| (16x the error of truncating accumulators), plus
-        # the rounding of the alpha product
-        e = 2.0 ** -20 * math.sqrt(L) * alpha * (T.abs() @ X.abs()) + 2.0 ** -22 * g64.abs()
-        del T
-        ratio = (ghat[b].double() - g64).abs() / e
-        assert not (ratio > 1).any() and torch.isfinite(ghat[b]).all(), f"gram_tx batch {b}: " + _worst_tile(ratio)
-        dot = (g64 * X).sum(1, keepdim=True)
-        nrm = norms[b].double()[:, None]
-        proj = (g64 - dot * X) / nrm
-        dot_err = (e * X.abs()).sum(1, keepdim=True) + C * 2.0 ** -23 * (g64 * X).abs().sum(1, keepdim=True)
-        tol = (e + X.abs() * dot_err + 2.0 ** -22 * (g64.abs() + (dot * X).abs())) / nrm
-        want = grad0[b].double().T + proj                                            # [L, C]
-        tol = tol + 2.0 ** -23 * want.abs()
-        for v, gr in grads.items():
-            ratio = (gr[b].double().T - want).abs() / tol
-            assert not (ratio > 1).any() and torch.isfinite(gr[b]).all(), \
-                f"gram_grad (FRESCO_GRAM_V={v}) batch {b}: " + _worst_tile(ratio)
+    A = None
     if dense:
         # the dense-target entry point (a caller holding the reference's fp32 correlation matrix): T = sign(G - A) +
-        # sign(G - A^T), loss over |G - A|; G from fp32 accumulation of C exact products, |G_kernel - G| <= C 2^-23
+        # sign(G - A^T), loss over |G - A|
         A = torch.empty(B, L, L, device="cuda")
         for b in range(B):
             A[b] = (xhat[b].double() @ xhat[b].double().T + 0.05 * torch.randn(L, L, device="cuda", generator=g,
                                                                                dtype=torch.float64)).float()
-        tsign2 = _nan((B, L, L), torch.float16)
-        loss2 = torch.zeros(1, device="cuda")
-        launch("fresco_gram_sign", fb.c.fresco_gram_sign(P(xhat), P(A), P(tsign2), P(loss2), B, L, C, weight, st))
-        band2, ref2 = C * 2.0 ** -22, 0.0
-        for b in range(B):
-            G = xhat[b].double() @ xhat[b].double().T
-            d1, d2 = G - A[b].double(), G - A[b].double().T
-            t = tsign2[b].double()
-            assert torch.isfinite(t).all(), f"dense target batch {b}: tsign not written"
-            bad = (t != torch.sign(d1) + torch.sign(d2)) & (d1.abs() > band2) & (d2.abs() > band2)
-            assert not bad.any(), f"dense target batch {b}: " + _worst_tile(bad.double() * 2)
-            ref2 += d1.abs().sum().item()
-        ref2 *= weight / (B * L * L)
-        assert abs(loss2.item() - ref2) < 1e-4 * ref2, (loss2.item(), ref2)
+        run.td_buf, run.tsign_d = True, _nan((B, L, L), torch.float16)
+        run.loss_d = torch.zeros(1, device="cuda")
+        launch("fresco_gram_sign", fb.c.fresco_gram_sign(P(xhat), P(A), P(run.tsign_d), P(run.loss_d), B, L, C, weight,
+                                                         st))
+    torch.cuda.synchronize()
+    GRB.check_run(run, xhat, yhat, norms, A, grad0, scale, torch.cuda.get_device_properties(0).multi_processor_count)
 
 
 _GRAM_KERNELS = ["gram_normalize_kernel", "gram_normalize_kernel", "gram2_kernel<G2_SIGN>", "gram2_kernel<G2_GRAD>",
