@@ -67,22 +67,27 @@ def _heads(t: torch.Tensor, heads: int) -> torch.Tensor:
     return t.double().reshape(B, L, heads, C // heads).transpose(1, 2)
 
 
-def _logits(q, k, heads, q_per_kv, scale, diag_bias):
-    """fp64 logits [B, H, Lq, Lk] (nats) and raw |q| . |k| row maxima, from the fp16 operands."""
+def _logits(q, k, heads, q_per_kv, scale, diag_bias, rows=None):
+    """fp64 logits [B, H, Lq, Lk] (nats) and raw |q| . |k| row maxima, from the fp16 operands.  ``rows`` (int64 [Lq]):
+    the absolute query index of each row of ``q`` when it is a subset of the rows, which the diagonal bias follows."""
     qh, kh = _heads(q, heads), _heads(k, heads).repeat_interleave(q_per_kv, 0)
     x = (qh @ kh.transpose(-1, -2)) * _f32(scale)
     bias = _f32(diag_bias)
     if bias != 0.0:
-        x = x + torch.eye(q.shape[1], k.shape[1], dtype=torch.float64, device=q.device) * bias
+        if rows is None:
+            diag = torch.eye(q.shape[1], k.shape[1], dtype=torch.float64, device=q.device)
+        else:
+            diag = (rows.to(q.device)[:, None] == torch.arange(k.shape[1], device=q.device)[None]).double()
+        x = x + diag * bias
     return x, qh, kh
 
 
-def ref_and_bound(q, k, v, heads, q_per_kv=1, scale=None, diag_bias=0.0, poly=0, rowsum=False):
-    """(attention_ref, attention_bound) in one pass, fp64 [B, Lq, H*d]."""
+def ref_and_bound(q, k, v, heads, q_per_kv=1, scale=None, diag_bias=0.0, poly=0, rowsum=False, rows=None):
+    """(attention_ref, attention_bound) in one pass, fp64 [B, Lq, H*d].  ``rows``: see ``_logits``."""
     B, Lq, C = q.shape
     d, Lk = C // heads, k.shape[1]
     scale = 1.0 / math.sqrt(d) if scale is None else scale
-    x, qh, kh = _logits(q, k, heads, q_per_kv, scale, diag_bias)
+    x, qh, kh = _logits(q, k, heads, q_per_kv, scale, diag_bias, rows)
     vh = _heads(v, heads).repeat_interleave(q_per_kv, 0)
     m = x.amax(-1, keepdim=True)
     e = torch.exp(x - m)

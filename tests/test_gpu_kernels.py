@@ -15,6 +15,7 @@ import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
+from oracle import attention_bound as AB  # noqa: E402  (checker only)
 from oracle import fresco_oracle as O  # noqa: E402  (checker only)
 from oracle import temporal_bound as TB  # noqa: E402  (checker only)
 from oracle import warp_chain_bound as CB  # noqa: E402  (checker only)
@@ -521,10 +522,12 @@ def test_config5_resolution_768(fb):
     k = torch.randn(chunks, Lk, C, device="cuda", generator=g).half()
     v = torch.randn(chunks, Lk, C, device="cuda", generator=g).half()
     out = fb.ops.attn_fwd(q, k, v, heads, N).float()
-    rows = [0, 127, 128, 4607, 9215]
+    rows = torch.tensor([0, 127, 128, 4607, 9215], device="cuda")
     for b in (0, 5):
-        ref = sdpa_ref(q[b:b + 1, rows], k[b // N:b // N + 1], v[b // N:b // N + 1], heads)
-        assert (out[b, rows] - ref[0]).abs().max().item() < 2e-3 * ref.abs().max().item()
+        # spot rows within the kernel's elementwise bound (oracle/attention_bound.py, the default variant)
+        ref, tol = AB.ref_and_bound(q[b:b + 1, rows], k[b // N:b // N + 1], v[b // N:b // N + 1], heads, rows=rows)
+        ratio = ((out[b:b + 1, rows].double() - ref).abs() / tol).nan_to_num(nan=float("inf"))
+        assert ratio.max().item() <= 1.0, (b, ratio.max().item())
     oc = fb.ops.attn_fwd(q, k, torch.full_like(v, -0.5), heads, N).float()
     assert (oc + 0.5).abs().max().item() < 1e-3
     # decoder features at 96x96 (768 / 8) and the image-resolution mapping at scale 8
