@@ -189,7 +189,8 @@ class FRESCOAttnProcessor2_0:
         from .dist import shard_layout
         layout = shard_layout(n_frames, self.shard)
         if layout.split_halves != (self._layout is not None and self._layout.split_halves) or (
-                layout.split_halves and (layout.world, layout.rank) != (self._layout.world, self._layout.rank)):
+                layout.split_halves and ((layout.world, layout.rank) != (self._layout.world, self._layout.rank)
+                                         or layout.group is not self._layout.group)):
             self._sharded = None
         self._layout = layout
 
@@ -437,13 +438,26 @@ def optimize_feature(sample, flows, occs, correlation_matrix=[], intra_weight=1e
     [chunks, C, h, w] fp32 per iteration).  The ranks hold the ``frame_range`` blocks of the batch, which need not be
     even; the batch frame count is that of ``flows`` (without flows: one all-reduce of the local counts).  The result
     is bit-identical to the unsharded call: the loss means run over the whole batch and the Gram kernels get the same
-    fp32 loss scale as unsharded (``ops.gram_*`` divide the rank's share of the weight in double and round once)."""
+    fp32 loss scale as unsharded (``ops.gram_*`` divide the rank's share of the weight in double and round once).
+
+    ``shard=dist.Box(...)`` takes the batch frame count from ``flows`` (a Box without them raises ValueError on every
+    rank): it picks the ranks the batch runs on, and an idle rank gets ``sample`` back at once."""
     have_temporal = flows is not None and occs is not None and optimize_temporal
     if (not have_temporal) and (intra_weight == 0 or len(correlation_matrix) == 0):
         return sample
     be = backend if backend is not None else _OptKernels()
     _, C, h, w = sample.shape
     world = 1 if shard is None else int(shard[0])
+    if world > 1:
+        from .dist import Box, shard_layout
+        if isinstance(shard, Box):
+            if flows is None:
+                raise ValueError("optimize_feature(shard=Box(...)) takes the batch's frame count from flows")
+            layout = shard_layout(int(flows[0].shape[0]), shard)
+            if layout.idle:
+                return sample
+            shard = layout.shard                        # the ranks the batch runs on
+            world = int(shard[0])
     comm = loss_comm = None
     split = False                       # this rank holds one CFG half (dist.shard_layout)
     chunks = unet_chunk_size
@@ -653,14 +667,17 @@ def get_intraframe_paras(pipe, imgs, frescoProc, prompt_embeds, do_classifier_fr
     the targets cover this rank's frames (both CFG chunks): what the sharded processor and
     ``optimize_feature(shard=...)`` take.  The pass is per frame, so no collective is issued.  With fewer frames than
     ranks (``dist.shard_layout``'s half layout) the pass runs on this rank's CFG half only, the targets cover its
-    samples, and the VAE posterior sample is drawn on the half-0 rank and sent to its partner."""
+    samples, and the VAE posterior sample is drawn on the half-0 ranks and sent to their peers.  An idle rank of a
+    ``dist.Box`` returns no targets at once."""
     from .dist import partner_share, shard_layout
+    B, C, H, W = imgs.shape
+    layout = shard_layout(B, shard)
+    if layout is not None and layout.idle:
+        return []
     scheduler = pipe.scheduler
     timestep = scheduler.timesteps[-1]
     device = pipe._execution_device
     generator = torch.Generator(device=device).manual_seed(seed)
-    B, C, H, W = imgs.shape
-    layout = shard_layout(B, shard)
     lo, hi = (0, B) if layout is None else (layout.lo, layout.hi)
     split = layout is not None and layout.split_halves
     chunks = 2 if do_classifier_free_guidance else 1
@@ -700,31 +717,38 @@ def get_flow_and_interframe_paras(flow_model, imgs, visualize_pipeline=False, sh
     pairs ``frame_range(N, world, rank)`` only and one all-gather (blocks padded to the largest share) assembles the
     whole batch's flows (rank order == pair order).  Occlusions, masks and trajectories are then built from the gathered flows on every rank, as unsharded:
     the return values are the whole batch's, as in the unsharded call.  With fewer frames than ranks
-    (``dist.shard_layout``'s half layout) the ranks of half 0 compute every pair once and each sends the gathered
-    flows to its partner: GMFlow is a network outside this library, whose bits could differ between two devices."""
+    (``dist.shard_layout``'s half and unequal-halves layouts) the ranks of half 0 compute every pair once and send
+    the flows of each pair to the half-1 ranks holding it, and each half gathers the whole batch's flows within
+    itself: GMFlow is a network outside this library, whose bits could differ between two devices.  An idle rank of a
+    ``dist.Box`` returns at once, with empty flows and occlusions, no masks and no trajectories."""
     from .dist import all_gather_frames, layout_group, partner_share, shard_layout
     from .flow_utils import flow_warp, forward_backward_consistency_check, get_mapping_ind
+    n = len(imgs)
+    layout = shard_layout(n, shard)
     param = next(flow_model.parameters())
     dev = param.device
+    if layout is not None and layout.idle:
+        h, w = imgs[0].shape[:2]
+        empty = torch.empty(0, 2, h, w, dtype=param.dtype, device=dev)
+        occ = torch.empty(0, h, w, dtype=torch.float32, device=dev)
+        return [empty, empty.clone()], [occ, occ.clone()], [], {"fwd_mappings": [], "bwd_mappings": [],
+                                                                 "interattn_masks": []}
     images = torch.stack([torch.from_numpy(im).permute(2, 0, 1).float() for im in imgs], dim=0).to(dev)
     imgs_torch = images / 127.5 - 1.0                                   # numpy2tensor (src/utils.py:8-12)
     reshuffle = list(range(1, len(images))) + [0]
-    n = len(images)
-    layout = shard_layout(n, shard)
     lo, hi = (0, n) if layout is None else (layout.lo, layout.hi)
 
     def flows():
         res = flow_model(images[lo:hi], images[reshuffle][lo:hi], attn_splits_list=[2], corr_radius_list=[-1],
                          prop_radius_list=[-1], pred_bidir_flow=True)
-        flow = res["flow_preds"][-1]                                    # [2 * pairs, 2, H, W]: forward | backward
-        grp = layout_group(layout)
-        if grp is not None:
-            flow = all_gather_frames(flow, n, grp[0], 2, grp[2])
-        return flow
+        return res["flow_preds"][-1]                                    # [2 * pairs, 2, H, W]: forward | backward
     if layout is not None and layout.split_halves:
-        flow = partner_share(layout, flows, ((2 * n, 2) + tuple(images.shape[2:]), param.dtype, dev))
+        flow = partner_share(layout, flows, ((2 * (hi - lo), 2) + tuple(images.shape[2:]), param.dtype, dev), chunks=2)
     else:
         flow = flows()
+    grp = layout_group(layout)
+    if grp is not None:
+        flow = all_gather_frames(flow, n, grp[0], 2, grp[2])
     fwd_flows, bwd_flows = flow.chunk(2)
     fwd_flows, bwd_flows = fwd_flows.contiguous(), bwd_flows.contiguous()
     fwd_occs, bwd_occs = forward_backward_consistency_check(fwd_flows, bwd_flows)

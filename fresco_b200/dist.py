@@ -4,7 +4,8 @@ The reference has no collective on this path (SURVEY 2.1); this module is the mu
 N keyframes of ONE batch are split contiguously over G ranks (rank r owns frames ``frame_range(N, G, r)`` =
 [r*N//G, (r+1)*N//G) of both CFG chunks; G need not divide N) and the UNet body runs as plain replicas.  A batch of
 G/2 <= N < G frames on an even G is split over the two CFG halves as well (``shard_layout``): every exchange below then
-runs with one chunk within the ranks of a half.  Only FRESCO attention couples frames:
+runs with one chunk within the ranks of a half.  A ``Box`` in place of the tuple also runs every other batch: unequal
+halves on an odd G, idle ranks beyond 2N.  Only FRESCO attention couples frames:
 
 * cross-frame attention (src/diffusion_hacked.py:225-247, :303-305): every query frame attends the same K/V set = all
   tokens of frame 0 + the occluded tokens of frames 1..N-1.  Each rank compacts the selected rows of ITS frames straight
@@ -47,21 +48,43 @@ def block_sizes(n_frames: int, world: int) -> List[int]:
     return [hi - lo for lo, hi in (frame_range(n_frames, world, r) for r in range(world))]
 
 
+class Box(tuple):
+    """``Box(world, rank, group=None)``: rank ``rank`` of ``world`` ranks (of ``group``, default: the whole world) that
+    may run a keyframe batch, as the ``shard`` argument of every sharded entry point.  It reads as the tuple
+    ``(world, rank, group)`` does, and ``shard_layout`` gives it the same frame and half layouts; where the tuple raises,
+    a Box still runs the batch: on an odd number of ranks the two CFG halves get ceil(G/2) and floor(G/2) ranks, and
+    ranks beyond 2N stay idle.  So one Box per rank runs every batch a driver makes, whatever its frame count."""
+
+    def __new__(cls, world: int, rank: int, group=None):
+        return tuple.__new__(cls, (int(world), int(rank), group))
+
+    def __repr__(self):
+        return f"Box(world={self[0]}, rank={self[1]}, group={self[2]!r})"
+
+
 class ShardLayout:
     """What one rank of a sharded keyframe batch holds and whom it exchanges with (``shard_layout``).
 
-    ``halves`` = [h0, h1): the CFG halves (0 unconditional, 1 text) of frames [``lo``, ``hi``) this rank holds.
-    ``world`` / ``rank`` / ``group``: the process group the frame-sharded exchanges (K/V all-gather, trajectory
-    all-to-alls, ring halo, warp re-shard, frame gathers) run on.  ``partner``: the global rank holding the other half
-    of the same frames, or None.  ``shard`` is the ``(world, rank, group)`` the caller passed."""
+    ``halves`` = [h0, h1): the CFG halves (0 unconditional, 1 text) of frames [``lo``, ``hi``) this rank holds; (0, 0)
+    on an idle rank, which holds nothing.  ``world`` / ``rank`` / ``group``: the process group the frame-sharded
+    exchanges (K/V all-gather, trajectory all-to-alls, ring halo, warp re-shard, frame gathers) run on.  ``peers``: (global
+    rank, lo, hi) of every rank of the other CFG half whose frames overlap this rank's, [lo, hi) the overlap;
+    ``partner``: the one peer when the two halves split alike, else None.  ``shard``: the ``(world, rank, group)`` or
+    ``Box`` of the ranks the batch runs on -- the caller's, or for a Box with idle ranks the Box of its first 2N."""
 
-    def __init__(self, n_frames, halves, lo, hi, world, rank, group, partner, shard):
+    def __init__(self, n_frames, halves, lo, hi, world, rank, group, partner, shard, peers=()):
         self.n_frames, self.halves, self.lo, self.hi = n_frames, halves, lo, hi
         self.world, self.rank, self.group, self.partner, self.shard = world, rank, group, partner, shard
+        self.peers = list(peers)
 
     @property
     def split_halves(self) -> bool:
-        return self.partner is not None
+        return self.halves[1] - self.halves[0] == 1
+
+    @property
+    def idle(self) -> bool:
+        """a rank of a Box beyond the 2N ranks the batch runs on"""
+        return self.halves[0] == self.halves[1]
 
     @property
     def half(self) -> int:
@@ -90,10 +113,11 @@ class ShardLayout:
 
     def __repr__(self):
         return (f"ShardLayout(n_frames={self.n_frames}, halves={self.halves}, frames=[{self.lo}, {self.hi}), "
-                f"world={self.world}, rank={self.rank}, partner={self.partner})")
+                f"world={self.world}, rank={self.rank}, peers={self.peers})")
 
 
 _HALF_GROUPS: dict = {}
+_ACTIVE_GROUPS: dict = {}
 
 
 def _global_rank(group, r: int) -> int:
@@ -107,29 +131,63 @@ def _splits_nccl(group) -> bool:
     return bool(getattr(dist.group.WORLD, "bound_device_id", None)) and dist.get_backend(group) == dist.Backend.NCCL
 
 
+def half_sizes(world: int) -> Tuple[int, int]:
+    """ranks of CFG half 0 and half 1 when ``world`` ranks split over the halves: ceil(G/2) and floor(G/2)"""
+    return world - world // 2, world // 2
+
+
+def _no_capture(what: str) -> None:
+    if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
+        raise RuntimeError(f"the {what} must exist before a step is captured: call a sharded entry point "
+                           "(get_flow_and_interframe_paras, get_intraframe_paras, inference) first")
+
+
 def half_group(world: int, rank: int, group=None):
     """The process group of the CFG half of rank ``rank`` of the shard group ``group`` (``world`` ranks): group ranks
-    [h*G/2, (h+1)*G/2) for h = rank // (G/2).  It depends on G and the shard's ranks only, is created on the first call
-    (every rank of the shard reaches its first half-layout entry point in the same order) and cached by the global
-    ranks of the shard, so a shard group made again over the same ranks finds it.  Only the shard's ranks take part:
-    under NCCL with a device-bound default group the shard group is split in two (``split_group``, collective over the
-    shard's ranks only: a plain ``new_group`` would split the default communicator, which needs every rank of the
-    world); otherwise each half is created by its own ranks (``new_group(..., use_local_synchronization=True)``)."""
-    per = world // 2
+    [0, G0) for half 0 and [G0, G) for half 1, G0 = ceil(G/2) (``half_sizes``); None for a half of one rank.  It
+    depends on G and the shard's ranks only, is created on the first call (every rank of the shard reaches its first
+    half-layout entry point in the same order) and cached by the global ranks of the shard, so a shard group made again
+    over the same ranks finds it.  Only the shard's ranks take part: under NCCL with a device-bound default group the
+    shard group is split in two (``split_group``, collective over the shard's ranks only: a plain ``new_group`` would
+    split the default communicator, which needs every rank of the world); otherwise each half is created by its own
+    ranks (``new_group(..., use_local_synchronization=True)``)."""
+    first = half_sizes(world)[0]
     shard_ranks = tuple(_global_rank(group, r) for r in range(world))
     if shard_ranks in _HALF_GROUPS:
         return _HALF_GROUPS[shard_ranks]
-    if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
-        raise RuntimeError("the CFG-half process groups must exist before a step is captured: call a sharded entry "
-                           "point (get_flow_and_interframe_paras, get_intraframe_paras, inference) first")
-    if per == 1:
+    _no_capture("CFG-half process groups")
+    halves = [list(range(first)), list(range(first, world))]
+    mine = halves[0 if rank < first else 1]
+    splits = [h for h in halves if len(h) > 1]                  # a half of one rank needs no group
+    if not splits:
         sub = None
     elif _splits_nccl(group):
-        sub = dist.split_group(parent_pg=group, split_ranks=[list(range(per)), list(range(per, world))])
+        sub = dist.split_group(parent_pg=group, split_ranks=splits)     # None on a rank in no split
     else:
-        h = rank // per
-        sub = dist.new_group(list(shard_ranks[h * per:(h + 1) * per]), use_local_synchronization=True)
+        sub = dist.new_group([shard_ranks[r] for r in mine], use_local_synchronization=True) if len(mine) > 1 else None
     _HALF_GROUPS[shard_ranks] = sub
+    return sub
+
+
+def active_group(world: int, rank: int, group, active: int):
+    """The process group of the first ``active`` ranks of the Box group ``group`` (``world`` ranks), the ranks a batch of
+    active/2 frames runs on; None on the other ranks.  Created on the first call and cached as ``half_group`` caches the
+    halves.  Under NCCL with a device-bound default group it is split from ``group`` (``split_group``), which every rank
+    of ``group`` enters once, the idle ones included; otherwise only the active ranks create it, and an idle rank
+    touches neither ``group`` nor any collective."""
+    if rank >= active and not _splits_nccl(group):
+        return None
+    if hasattr(group, "sub_comm"):
+        return group.sub_comm(active, rank)                     # an injected communicator (tests) supplies its own
+    key = (tuple(_global_rank(group, r) for r in range(world)), active)
+    if key in _ACTIVE_GROUPS:
+        return _ACTIVE_GROUPS[key]
+    _no_capture("process group of a Box's active ranks")
+    if _splits_nccl(group):
+        sub = dist.split_group(parent_pg=group, split_ranks=[list(range(active))])
+    else:
+        sub = dist.new_group(list(key[0][:active]), use_local_synchronization=True)
+    _ACTIVE_GROUPS[key] = sub
     return sub
 
 
@@ -142,29 +200,47 @@ def shard_layout(n_frames: int, shard) -> Optional[ShardLayout]:
     * G even and G/2 <= N < G: the half layout -- rank r holds half r // (G/2) of frames ``frame_range(N, G/2, r %
       (G/2))``; the exchanges run on the group of its half (``half_group``); its partner r +- G/2 holds the other half
       of the same frames.
-    * otherwise: ValueError."""
+    * otherwise: ValueError for a tuple.  A ``Box`` goes on:
+      * G odd and N < G <= 2N: the unequal-halves layout -- half 0 gets the first G0 = ceil(G/2) ranks, half 1 the other
+        G1 = floor(G/2); rank r of half h holds frames ``frame_range(N, G_h, r - h*G0)`` of that half, the exchanges run
+        on the group of its half, and its ``peers`` are the ranks of the other half whose frames overlap its own.
+      * G > 2N: the first 2N ranks run the batch in the half layout, on their own process group (``active_group``);
+        the others get an idle layout and take part in nothing."""
     if shard is None:
         return None
     if isinstance(shard, ShardLayout):
         return shard
     world, rank = int(shard[0]), int(shard[1])
     group = shard[2] if len(shard) > 2 else None
+    box = isinstance(shard, Box)
+    if box and world > 2 * n_frames:
+        active = 2 * n_frames
+        sub = active_group(world, rank, group, active)
+        if rank >= active:
+            return ShardLayout(n_frames, (0, 0), 0, 0, 1, 0, None, None, shard)
+        return shard_layout(n_frames, Box(active, rank, sub))
     if n_frames >= world:
         lo, hi = frame_range(n_frames, world, rank)
         return ShardLayout(n_frames, (0, 2), lo, hi, world, rank, group, None, shard)
-    if world % 2 != 0 or 2 * n_frames < world:
+    if (world % 2 != 0 and not box) or 2 * n_frames < world:
         raise ValueError(f"{n_frames} frames cannot be sharded over {world} ranks: shard over the two guidance halves "
                          f"needs an even number of ranks G <= 2N = {2 * n_frames}, or run the batch on a process group "
                          f"of {n_frames} ranks, shard=({n_frames}, rank, group)")
-    per = world // 2
-    h, r = rank // per, rank % per
-    lo, hi = frame_range(n_frames, per, r)
-    if hasattr(group, "half_comm"):
-        # an injected communicator (tests: ranks as threads) supplies the communicator of the half itself
-        sub, partner = group.half_comm(world, rank), (1 - h) * per + r
-    else:
-        sub, partner = half_group(world, rank, group), _global_rank(group, (1 - h) * per + r)
-    return ShardLayout(n_frames, (h, h + 1), lo, hi, per, r, sub, partner, shard)
+    sizes = half_sizes(world)
+    h = 0 if rank < sizes[0] else 1
+    r = rank - h * sizes[0]
+    lo, hi = frame_range(n_frames, sizes[h], r)
+    injected = hasattr(group, "half_comm")
+    # an injected communicator (tests: ranks as threads) supplies the communicator of the half itself
+    sub = group.half_comm(world, rank) if injected else half_group(world, rank, group)
+    peers = []
+    for s in range(sizes[1 - h]):                               # the other half's ranks whose frames overlap mine
+        a, b = frame_range(n_frames, sizes[1 - h], s)
+        if max(a, lo) < min(b, hi):
+            peer = (1 - h) * sizes[0] + s
+            peers.append((peer if injected else _global_rank(group, peer), max(a, lo), min(b, hi)))
+    partner = peers[0][0] if sizes[0] == sizes[1] else None
+    return ShardLayout(n_frames, (h, h + 1), lo, hi, sizes[h], r, sub, partner, shard, peers)
 
 
 def layout_group(layout: Optional[ShardLayout]):
@@ -189,27 +265,57 @@ def send_recv(sends, recvs, group=None) -> None:
             dst.copy_(src)
 
 
+def _peer_rows(t: torch.Tensor, chunks: int, n: int, a: int, b: int) -> torch.Tensor:
+    """rows of frames [a, b) (counted from the rank's first frame) of each chunk of ``t = [chunks * n, ...]``"""
+    if chunks == 1:
+        return t[a:b]
+    return t.view((chunks, n) + tuple(t.shape[1:]))[:, a:b]
+
+
+def _cross_halves(layout: ShardLayout, send: Optional[torch.Tensor], recv: Optional[torch.Tensor], chunks: int) -> None:
+    """One batched ``send_recv`` with the peers of ``layout`` (the other CFG half's ranks whose frames overlap this
+    rank's): each gets the rows of ``send`` of the frames it shares with this rank, and the rows of ``recv`` of those
+    frames are filled from it.  ``send`` / ``recv`` are ``(chunk, frame)``-major ``[chunks * n_local, ...]``; every size
+    is a host int of the layout, so nothing reads from the device."""
+    n = layout.hi - layout.lo
+    sends, recvs, copies = [], [], []
+    for peer, a, b in layout.peers:
+        a, b = a - layout.lo, b - layout.lo
+        if send is not None:
+            sends.append((_peer_rows(send, chunks, n, a, b).contiguous(), peer))
+        if recv is not None:
+            dst = _peer_rows(recv, chunks, n, a, b)
+            buf = dst if dst.is_contiguous() else torch.empty(dst.shape, dtype=dst.dtype, device=dst.device)
+            recvs.append((buf, peer))
+            copies.append((dst, buf))
+    send_recv(sends, recvs, layout.shard[2] if len(layout.shard) > 2 else None)
+    for dst, buf in copies:
+        if buf is not dst:
+            dst.copy_(buf)
+
+
 def partner_swap(layout: ShardLayout, mine: torch.Tensor) -> torch.Tensor:
-    """The partner's tensor of the same shape and dtype as ``mine``: one batched send / receive pair (``send_recv``,
-    as ``RingComm.shift``)."""
+    """The other CFG half's rows of this rank's frames, shaped as ``mine`` ([n_local, ...]): one batched send / receive
+    with every peer (``send_recv``, as ``RingComm.shift``) -- in the half layout, the partner's whole tensor."""
     mine = mine.contiguous()
     theirs = torch.empty_like(mine)
-    send_recv([(mine, layout.partner)], [(theirs, layout.partner)], layout.shard[2] if len(layout.shard) > 2 else None)
+    _cross_halves(layout, mine, theirs, 1)
     return theirs
 
 
-def partner_share(layout: ShardLayout, make, like: Tuple[tuple, torch.dtype, torch.device]) -> torch.Tensor:
-    """What ``make()`` returns, computed once on the half-0 rank and sent to its partner, which receives it into a
-    tensor of ``like = (shape, dtype, device)`` without calling ``make``.  Used for everything drawn from an unseeded
-    generator or computed by a network outside this library, whose bits could differ between two devices."""
-    group = layout.shard[2] if len(layout.shard) > 2 else None
+def partner_share(layout: ShardLayout, make, like: Tuple[tuple, torch.dtype, torch.device], chunks: int = 1) -> torch.Tensor:
+    """What ``make()`` returns for this rank's frames ([chunks * n_local, ...], ``(chunk, frame)``-major), computed once
+    on the ranks of half 0, each of which sends every peer the rows of the frames they share; a half-1 rank receives
+    its rows into a tensor of ``like = (shape, dtype, device)`` without calling ``make``.  Used for everything drawn
+    from an unseeded generator or computed by a network outside this library, whose bits could differ between two
+    devices."""
     if layout.half == 0:
         out = make().contiguous()
-        send_recv([(out, layout.partner)], [], group)
+        _cross_halves(layout, out, None, chunks)
     else:
         shape, dtype, device = like
         out = torch.empty(shape, dtype=dtype, device=device)
-        send_recv([], [(out, layout.partner)], group)
+        _cross_halves(layout, None, out, chunks)
     return out
 
 

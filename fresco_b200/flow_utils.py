@@ -126,8 +126,9 @@ def warp_tensor(sample, flows, occs, saliency, unet_chunk_size, shard=None):
 
     ``shard=(world, rank[, group])`` (not in the reference): ``sample`` holds this rank's frames of a frame-sharded
     batch (flows / occs / saliency describe ALL N frames).  With fewer frames than ranks (``dist.shard_layout``'s half
-    layout) ``sample`` holds one CFG half of this rank's frames, [n_local, ...] whatever ``unet_chunk_size`` says,
-    and everything below runs within the ranks of that half (``shard`` may also be the ``ShardLayout`` itself).  The
+    and unequal-halves layouts) ``sample`` holds one CFG half of this rank's frames, [n_local, ...] whatever
+    ``unet_chunk_size`` says, and everything below runs within the ranks of that half (``shard`` may also be the
+    ``ShardLayout`` itself); an idle rank of a ``dist.Box`` gets ``sample`` back.  The
     chain is sequential over frames but independent per (chunk, channel) plane, so the batch is re-sharded by CHANNEL
     for the chain: one all-to-all turns
     [frames/G, all channels] into [all frames, channels/G], every rank runs the chain kernel on its channel slice, a
@@ -138,6 +139,8 @@ def warp_tensor(sample, flows, occs, saliency, unet_chunk_size, shard=None):
     if shard is not None:
         from .dist import shard_layout
         layout = shard_layout(flows[0].shape[0], shard)
+        if layout.idle:
+            return sample                                       # an idle rank of a dist.Box holds no frame
         if layout.world == 1 and not layout.split_halves:
             layout = None                                       # one rank: the unsharded call
     world = 1 if layout is None else layout.world

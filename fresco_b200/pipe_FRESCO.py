@@ -22,7 +22,7 @@ from typing import List, Optional
 import torch
 
 from . import ops
-from .dist import layout_group, partner_share, partner_swap, shard_layout
+from .dist import Box, layout_group, partner_share, partner_swap, shard_layout
 from .flow_utils import warp_tensor
 
 
@@ -52,10 +52,19 @@ def step(pipe, model_output, timestep, sample, generator, repeat_noise=False, vi
     ``noise`` (optional) replaces the ``torch.randn`` draw of :61-62 (the frame-sharded loop passes its slice).
     ``shard=(world, rank[, group])``: ``sample`` holds this rank's frames of a frame-sharded batch (``flows`` / ``occs``
     / ``saliency`` the whole batch's); background smoothing decodes and re-encodes those frames only and warps them
-    along the whole chain.  ``shard`` may be a ``dist.ShardLayout``; in its half layout ``model_output`` is this rank's
-    CFG half of the raw UNet output [n, ...]: it is swapped with the partner's (one send / receive pair) so both run the
-    guidance on the same [uncond; text] operands, and the smoothing round trip runs on the ranks of half 0, which send
-    its result to their partners."""
+    along the whole chain.  ``shard`` may be a ``dist.ShardLayout``; in its half and unequal-halves layouts
+    ``model_output`` is this rank's CFG half of the raw UNet output [n, ...]: the other half's rows of the same frames
+    come from the peers (one batched send / receive), so every rank runs the guidance on a contiguous [uncond; text]
+    block, and the smoothing round trip runs on the ranks of half 0, which send its rows to their peers.  On an idle
+    rank of a ``dist.Box`` it returns ``(sample, sample)`` at once.  A ``dist.Box`` itself takes the frame count from
+    ``flows``; without them, pass its layout (``dist.shard_layout(N, box)``), as ``inference`` does."""
+    if isinstance(shard, Box):
+        if flows is None:
+            raise ValueError("step(shard=Box(...)) without flows does not know the batch's frame count: pass "
+                             "dist.shard_layout(n_frames, box)")
+        shard = shard_layout(int(flows[0].shape[0]), shard)
+    if getattr(shard, "idle", False):
+        return (sample, sample)
     alpha_prod_t, c_x0, c_xt, sigma = _step_coefficients(pipe.scheduler, timestep)
     sample = sample.contiguous()
     do_cfg = guidance_scale is not None
@@ -107,14 +116,22 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
 
     ``imgs`` / ``edges`` / ``prompt_embeds`` / ``flows`` / ``occs`` / ``saliency`` hold ALL N frames (every rank gets the
     same arguments); with ``shard=(world, rank[, group])`` this rank denoises frames [rank*N//G, (rank+1)*N//G) and
-    returns their latents, the background-smoothing steps included."""
+    returns their latents, the background-smoothing steps included.  With ``shard=dist.Box(...)`` every frame count
+    runs (``dist.shard_layout``); an idle rank returns empty latents [0, 4, h, w] at once and leaves ``record_latents``
+    as it is."""
     device = pipe._execution_device
     noise_scheduler = pipe.scheduler
-    generator = torch.Generator(device=device).manual_seed(seed)
     B, C, H, W = imgs.shape
     layout = shard_layout(B, shard)
+    if layout is not None and layout.idle:
+        f = getattr(pipe, "vae_scale_factor", 8)
+        return torch.empty(0, pipe.unet.config.in_channels, H // f, W // f, dtype=prompt_embeds.dtype, device=device)
+    generator = torch.Generator(device=device).manual_seed(seed)
     lo, hi = (0, B) if layout is None else (layout.lo, layout.hi)
     split = layout is not None and layout.split_halves
+    chunks = 2 if do_classifier_free_guidance else 1
+    if split:
+        layout.chunks(chunks)                                                   # the halves need both CFG halves
     if hasattr(frescoProc, "set_batch_frames"):
         frescoProc.set_batch_frames(B)
     latents = pipe.prepare_latents(B, pipe.unet.config.in_channels, H, W, prompt_embeds.dtype, device, generator,
@@ -132,9 +149,6 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
                                                    latents.device)) if split else encode()
         latents_init = noise_scheduler.add_noise(latent_x0, latents[lo:hi], timesteps[num_warmup_steps]).detach()
     n_local = hi - lo
-    chunks = 2 if do_classifier_free_guidance else 1
-    if split:
-        layout.chunks(chunks)                                                   # the half layout needs both CFG halves
     pe = prompt_embeds if layout is None else layout.rows(prompt_embeds, chunks)    # (b f) layout: the frames held
     gather = layout_group(layout)                                               # record_latents: within the half
     sub_flows = sub_occs = sub_sal = None
@@ -145,11 +159,16 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
         if t < step_interattn_end:
             frescoProc.controller.disable_interattn()
         if propagation_mode:                                                     # :175-177
-            rec = record_latents[i].detach().clone()
-            for f in range(2):
-                if lo <= f < hi:
-                    latents[f - lo] = rec[f]
-            record_latents[i] = _gather_first_last(latents, B, lo, hi, gather)
+            if lo < 2:                                                           # this rank holds frame 0 or 1
+                rec = record_latents[i].detach().clone()
+                for f in range(2):
+                    if lo <= f < hi:
+                        latents[f - lo] = rec[f]
+            first_last = _gather_first_last(latents, B, lo, hi, gather)
+            if i < len(record_latents):
+                record_latents[i] = first_last
+            else:                                                                # idle in the first batch of a Box
+                record_latents.append(first_last)
         else:
             record_latents += [_gather_first_last(latents, B, lo, hi, gather)]
         # one CFG half per rank in the half layout: its latents, prompt and edge rows only
@@ -172,5 +191,5 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
         latents = step(pipe, noise_pred, t, latents, generator, visualize_pipeline=visualize_pipeline,
                        flows=flows if smooth else None, occs=occs if smooth else None, saliency=saliency if smooth else None,
                        guidance_scale=guidance_scale if do_classifier_free_guidance else None, noise=noise,
-                       shard=layout if split else shard)[0]
+                       shard=layout)[0]
     return latents
