@@ -23,6 +23,7 @@ import torch.nn.functional as F
 
 from . import ops
 from ._lib import FrescoError
+from .dist import ShardedFRESCOAttention, batch_layout, shard_layout, unpack
 from .flow_utils import adjoint_csr, clear_prep_cache, resize_flows_occs, warp_tensor
 
 
@@ -179,6 +180,8 @@ class FRESCOAttnProcessor2_0:
         self.shard = shard
         self._sharded = None
         self._layout = None
+        # (world, rank, group, chunks) the sharded layer runs on: the frame layout of ``shard`` until a batch says otherwise
+        self._layer_key = None if shard is None else unpack(shard) + (unet_chunk_size,)
 
     def set_batch_frames(self, n_frames: int) -> None:
         """Tell a sharded processor the frame count of the keyframe batch it runs on (``inference`` and
@@ -186,13 +189,11 @@ class FRESCOAttnProcessor2_0:
         of that half (``dist.shard_layout``).  Without a call, the frame layout is assumed."""
         if self.shard is None:
             return
-        from .dist import shard_layout
         layout = shard_layout(n_frames, self.shard)
-        if layout.split_halves != (self._layout is not None and self._layout.split_halves) or (
-                layout.split_halves and ((layout.world, layout.rank) != (self._layout.world, self._layout.rank)
-                                         or layout.group is not self._layout.group)):
+        key = (layout.world, layout.rank, layout.group, layout.chunks(self.unet_chunk_size))
+        if key != self._layer_key:
             self._sharded = None
-        self._layout = layout
+        self._layout, self._layer_key = layout, key
 
     def __call__(self, attn, hidden_states, encoder_hidden_states=None, attention_mask=None, temb=None):
         residual = hidden_states
@@ -251,14 +252,7 @@ class FRESCOAttnProcessor2_0:
         v = value.to(torch.float16).contiguous()
         if self.shard is not None and ctrl is not None:
             if self._sharded is None:
-                from .dist import ShardedFRESCOAttention
-                layout = self._layout
-                if layout is not None and layout.split_halves:
-                    # one CFG half: chunks = 1, the exchanges (and the no-mask frame-0 broadcast) within the half
-                    world, rank, group = layout.world, layout.rank, layout.group
-                    chunks = layout.chunks(self.unet_chunk_size)
-                else:
-                    (world, rank, group), chunks = self.shard, self.unet_chunk_size
+                world, rank, group, chunks = self._layer_key
                 self._sharded = ShardedFRESCOAttention(ctrl, world, rank, chunks, group)
             ref_q = ref_k = None
             if ctrl.use_intraattn:
@@ -445,62 +439,27 @@ def optimize_feature(sample, flows, occs, correlation_matrix=[], intra_weight=1e
     have_temporal = flows is not None and occs is not None and optimize_temporal
     if (not have_temporal) and (intra_weight == 0 or len(correlation_matrix) == 0):
         return sample
+    layout = batch_layout(shard, flows, sample, unet_chunk_size,
+                          "optimize_feature(shard=Box(...)) takes the batch's frame count from flows", count=True)
+    if layout.idle:
+        return sample
     be = backend if backend is not None else _OptKernels()
     _, C, h, w = sample.shape
-    world = 1 if shard is None else int(shard[0])
-    if world > 1:
-        from .dist import Box, shard_layout
-        if isinstance(shard, Box):
-            if flows is None:
-                raise ValueError("optimize_feature(shard=Box(...)) takes the batch's frame count from flows")
-            layout = shard_layout(int(flows[0].shape[0]), shard)
-            if layout.idle:
-                return sample
-            shard = layout.shard                        # the ranks the batch runs on
-            world = int(shard[0])
-    comm = loss_comm = None
-    split = False                       # this rank holds one CFG half (dist.shard_layout)
-    chunks = unet_chunk_size
+    chunks = layout.chunks(unet_chunk_size)
     n = sample.shape[0] // chunks
-    lo, total = 0, n
-    mean_frames = None                  # total_frames of the temporal mean (None: this call's frames)
-    if world > 1:
-        from .dist import RingComm, shard_layout
-        rank = int(shard[1])
-        third = shard[2] if len(shard) > 2 else None
-        loss_comm = third if hasattr(third, "shift") else RingComm(world, rank, third)
-        if flows is not None:
-            total = int(flows[0].shape[0])
-        else:
-            # every (chunk, frame) sample is held once in either layout: the batch has (all rows) / chunks frames
-            count = torch.full((1,), sample.shape[0], dtype=torch.int64, device=sample.device)
-            loss_comm.all_reduce_sum(count)
-            total = int(count.item()) // unet_chunk_size
-        layout = shard_layout(total, shard)
-        chunks = layout.chunks(unet_chunk_size)
-        n = sample.shape[0] // chunks
-        lo, hi = layout.lo, layout.hi
-        if hi - lo != n or sample.shape[0] != chunks * n:
-            raise FrescoError("optimize_feature: %r owns frames [%d, %d) of the %d-frame batch, got %d rows"
-                              % (layout, lo, hi, total, sample.shape[0]))
-        split = layout.split_halves
-        if split:
-            # the ring of this rank's CFG half; the loss trace still sums over the whole shard
-            sub = layout.group
-            comm = sub if hasattr(sub, "shift") else RingComm(layout.world, layout.rank, sub) if layout.world > 1 else None
-            # the halo kernel forms the mean's element count as chunks * total_frames * C*h*w in double: one chunk and
-            # 2N "frames" give the unsharded 2 * N * C*h*w exactly
-            mean_frames = 2 * total
-        else:
-            comm = loss_comm
-            mean_frames = total
+    lo, hi, total = layout.lo, layout.hi, layout.n_frames
+    if hi - lo != n or sample.shape[0] != chunks * n:
+        raise FrescoError("optimize_feature: %r owns frames [%d, %d) of the %d-frame batch, got %d rows"
+                          % (layout, lo, hi, total, sample.shape[0]))
+    ring = layout.ring()                # the halo exchange of this rank's frame ring (None: the ring is closed here)
+    trace_comm = layout.trace_comm()    # the loss trace sums over the whole shard
     cs = sample.to(torch.float32).reshape(chunks, n, C, h, w).contiguous().clone()
     grad = torch.empty_like(cs)
     exp_avg = torch.zeros_like(cs)
     exp_avg_sq = torch.zeros_like(cs)
     if have_temporal:
-        prep = be.temporal_prepare(flows, occs, h, lo, lo + n, total)
-        if comm is not None:
+        prep = be.temporal_prepare(flows, occs, h, lo, hi, total)
+        if ring is not None:
             first, halo_cs, halo_grad, from_prev = (torch.empty(chunks, C, h, w, dtype=torch.float32,
                                                                 device=sample.device) for _ in range(4))
     target = None
@@ -513,25 +472,19 @@ def optimize_feature(sample, flows, occs, correlation_matrix=[], intra_weight=1e
         target = target.to(torch.float32).contiguous()
     # F.l1_loss averages over the frames of the WHOLE batch: a rank's share of the weight, which the Gram kernels divide
     # by this rank's batch in double (ops.gram_*), so the fp32 loss scale is the unsharded one
-    # (a rank holding one CFG half has n of the 2N samples)
-    if split:
-        weight = intra_weight * (float(n) / float(2 * total))
-    else:
-        weight = intra_weight * (float(n) / float(total))
+    weight = intra_weight * layout.row_share
     loss_acc = torch.zeros(1, dtype=torch.float32, device=sample.device) if trace is not None else None
     for it in range(1, iters + 1):
         if loss_acc is not None:
             loss_acc.zero_()
-        if have_temporal and comm is not None:
+        if have_temporal and ring is not None:
             first.copy_(cs[:, 0])
-            comm.shift(first, halo_cs, -1)                      # my first frame is the previous rank's halo
-            be.temporal(cs, prep, grad, loss_acc, halo_cs, halo_grad, mean_frames)
-            comm.shift(halo_grad, from_prev, +1)                # what my first frame receives from the previous rank's last pair
+            ring.shift(first, halo_cs, -1)                      # my first frame is the previous rank's halo
+            be.temporal(cs, prep, grad, loss_acc, halo_cs, halo_grad, layout.mean_frames)
+            ring.shift(halo_grad, from_prev, +1)                # what my first frame receives from the previous rank's last pair
             grad[:, 0] += from_prev
-        elif have_temporal and mean_frames is not None:
-            be.temporal(cs, prep, grad, loss_acc, total_frames=mean_frames)     # one CFG half on a one-rank half group
         elif have_temporal:
-            be.temporal(cs, prep, grad, loss_acc)
+            be.temporal(cs, prep, grad, loss_acc, total_frames=layout.mean_frames)
         else:
             grad.zero_()
         if spatial:
@@ -539,8 +492,8 @@ def optimize_feature(sample, flows, occs, correlation_matrix=[], intra_weight=1e
                        loss_acc)
         be.adam(cs, grad, exp_avg, exp_avg_sq, it)
         if trace is not None:
-            if loss_comm is not None:
-                loss_comm.all_reduce_sum(loss_acc)
+            if trace_comm is not None:
+                trace_comm.all_reduce_sum(loss_acc)
             trace.losses.append(float(loss_acc.item()))
     return be.adain(cs.view(chunks * n, C, h, w), sample)
 
@@ -583,8 +536,7 @@ def my_forward(self, steps=[], layers=[0, 1, 2, 3], flows=None, occs=None, corre
                 # frame-sharded batch (shard != None): optimize_feature exchanges one boundary frame per Adam iteration
                 # with its ring neighbours, warp_tensor re-shards the chain by channel
                 new = optimize_feature(feat, flows, occs, correlation_matrix, intra_weight, iters,
-                                       optimize_temporal=optimize_temporal,
-                                       shard=shard if (shard is not None and shard[0] > 1) else None)
+                                       optimize_temporal=optimize_temporal, shard=shard)
                 if saliency is not None:
                     new = warp_tensor(new, flows, occs, saliency, 2, shard=shard)
                 if "hidden_states" in h_kwargs:
@@ -669,20 +621,16 @@ def get_intraframe_paras(pipe, imgs, frescoProc, prompt_embeds, do_classifier_fr
     ranks (``dist.shard_layout``'s half layout) the pass runs on this rank's CFG half only, the targets cover its
     samples, and the VAE posterior sample is drawn on the half-0 ranks and sent to their peers.  An idle rank of a
     ``dist.Box`` returns no targets at once."""
-    from .dist import partner_share, shard_layout
     B, C, H, W = imgs.shape
     layout = shard_layout(B, shard)
-    if layout is not None and layout.idle:
+    if layout.idle:
         return []
     scheduler = pipe.scheduler
     timestep = scheduler.timesteps[-1]
     device = pipe._execution_device
     generator = torch.Generator(device=device).manual_seed(seed)
-    lo, hi = (0, B) if layout is None else (layout.lo, layout.hi)
-    split = layout is not None and layout.split_halves
-    chunks = 2 if do_classifier_free_guidance else 1
-    if split:
-        layout.chunks(chunks)                                       # the half layout needs both CFG halves
+    lo, hi = layout.lo, layout.hi
+    chunks = layout.chunks(2 if do_classifier_free_guidance else 1)     # the half layout needs both CFG halves
     if hasattr(frescoProc, "set_batch_frames"):
         frescoProc.set_batch_frames(B)
     ctrl = frescoProc.controller
@@ -695,11 +643,10 @@ def get_intraframe_paras(pipe, imgs, frescoProc, prompt_embeds, do_classifier_fr
 
     def encode():
         return pipe.vae.config.scaling_factor * pipe.vae.encode(imgs[lo:hi].to(pipe.unet.dtype)).latent_dist.sample()
-    latent_x0 = (partner_share(layout, encode, (latents.shape, getattr(pipe.vae, "dtype", pipe.unet.dtype), latents.device))
-                 if split else encode())
+    latent_x0 = layout.share(encode, (latents.shape, getattr(pipe.vae, "dtype", pipe.unet.dtype), latents.device))
     latents = scheduler.add_noise(latent_x0, latents, timestep).detach()
-    model_in = torch.cat([latents] * 2) if do_classifier_free_guidance and not split else latents
-    pe = prompt_embeds if layout is None else layout.rows(prompt_embeds, chunks)
+    model_in = torch.cat([latents] * chunks) if chunks > 1 else latents
+    pe = layout.rows(prompt_embeds, 2 if do_classifier_free_guidance else 1)
     out = pipe.unet(model_in, timestep, encoder_hidden_states=pe, cross_attention_kwargs=None, return_dict=False)
     ctrl.disable_store()
     return gram_targets(out[1:])
@@ -721,13 +668,12 @@ def get_flow_and_interframe_paras(flow_model, imgs, visualize_pipeline=False, sh
     the flows of each pair to the half-1 ranks holding it, and each half gathers the whole batch's flows within
     itself: GMFlow is a network outside this library, whose bits could differ between two devices.  An idle rank of a
     ``dist.Box`` returns at once, with empty flows and occlusions, no masks and no trajectories."""
-    from .dist import all_gather_frames, layout_group, partner_share, shard_layout
     from .flow_utils import flow_warp, forward_backward_consistency_check, get_mapping_ind
     n = len(imgs)
     layout = shard_layout(n, shard)
     param = next(flow_model.parameters())
     dev = param.device
-    if layout is not None and layout.idle:
+    if layout.idle:
         h, w = imgs[0].shape[:2]
         empty = torch.empty(0, 2, h, w, dtype=param.dtype, device=dev)
         occ = torch.empty(0, h, w, dtype=torch.float32, device=dev)
@@ -736,19 +682,14 @@ def get_flow_and_interframe_paras(flow_model, imgs, visualize_pipeline=False, sh
     images = torch.stack([torch.from_numpy(im).permute(2, 0, 1).float() for im in imgs], dim=0).to(dev)
     imgs_torch = images / 127.5 - 1.0                                   # numpy2tensor (src/utils.py:8-12)
     reshuffle = list(range(1, len(images))) + [0]
-    lo, hi = (0, n) if layout is None else (layout.lo, layout.hi)
+    lo, hi = layout.lo, layout.hi
 
     def flows():
         res = flow_model(images[lo:hi], images[reshuffle][lo:hi], attn_splits_list=[2], corr_radius_list=[-1],
                          prop_radius_list=[-1], pred_bidir_flow=True)
         return res["flow_preds"][-1]                                    # [2 * pairs, 2, H, W]: forward | backward
-    if layout is not None and layout.split_halves:
-        flow = partner_share(layout, flows, ((2 * (hi - lo), 2) + tuple(images.shape[2:]), param.dtype, dev), chunks=2)
-    else:
-        flow = flows()
-    grp = layout_group(layout)
-    if grp is not None:
-        flow = all_gather_frames(flow, n, grp[0], 2, grp[2])
+    flow = layout.share(flows, ((2 * (hi - lo), 2) + tuple(images.shape[2:]), param.dtype, dev), chunks=2)
+    flow = layout.gather_frames(flow, 2)
     fwd_flows, bwd_flows = flow.chunk(2)
     fwd_flows, bwd_flows = fwd_flows.contiguous(), bwd_flows.contiguous()
     fwd_occs, bwd_occs = forward_backward_consistency_check(fwd_flows, bwd_flows)

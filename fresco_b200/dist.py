@@ -70,7 +70,10 @@ class ShardLayout:
     exchanges (K/V all-gather, trajectory all-to-alls, ring halo, warp re-shard, frame gathers) run on.  ``peers``: (global
     rank, lo, hi) of every rank of the other CFG half whose frames overlap this rank's, [lo, hi) the overlap;
     ``partner``: the one peer when the two halves split alike, else None.  ``shard``: the ``(world, rank, group)`` or
-    ``Box`` of the ranks the batch runs on -- the caller's, or for a Box with idle ranks the Box of its first 2N."""
+    ``Box`` of the ranks the batch runs on -- the caller's, or for a Box with idle ranks the Box of its first 2N.
+
+    The one-rank layout (``shard_layout(n, None)``) holds everything and exchanges nothing; every method below then
+    does what an unsharded call does."""
 
     def __init__(self, n_frames, halves, lo, hi, world, rank, group, partner, shard, peers=()):
         self.n_frames, self.halves, self.lo, self.hi = n_frames, halves, lo, hi
@@ -90,6 +93,17 @@ class ShardLayout:
     def half(self) -> int:
         """the CFG half this rank holds in the half layout"""
         return self.halves[0]
+
+    @property
+    def row_share(self) -> float:
+        """rows held / rows in the batch: this rank's share of a loss averaged over the whole batch"""
+        return float((self.hi - self.lo) * (self.halves[1] - self.halves[0])) / float(2 * self.n_frames)
+
+    @property
+    def mean_frames(self) -> int:
+        """the frame count of the temporal loss's mean in the element count chunks * frames * C*h*w, chunks being this
+        rank's: N with both CFG halves, 2N with one, so that the count is the unsharded call's"""
+        return self.n_frames * 2 // (self.halves[1] - self.halves[0])
 
     def chunks(self, cfg_chunks: int) -> int:
         """CFG chunks of this rank's rows for a call that would hold ``cfg_chunks`` unsharded"""
@@ -111,9 +125,74 @@ class ShardLayout:
         base = self.half * self.n_frames
         return t[base + self.lo:base + self.hi]
 
+    def guided(self, model_output: torch.Tensor, do_cfg: bool) -> torch.Tensor:
+        """The raw UNet output of both CFG halves of this rank's frames, [uncond; text], from this rank's: as it is when
+        the rank holds both halves; in the half layouts its rows and the peers' (``swap``), in half order."""
+        if not self.split_halves:
+            return model_output
+        if not do_cfg:
+            raise ValueError("a batch sharded over the CFG halves needs guidance_scale")
+        mine = model_output.contiguous()
+        theirs = self.swap(mine)
+        return torch.cat([mine, theirs] if self.half == 0 else [theirs, mine])
+
+    def swap(self, mine: torch.Tensor) -> torch.Tensor:
+        """The other CFG half's rows of this rank's frames, shaped as ``mine`` ([n_local, ...]): one batched send /
+        receive with every peer (``send_recv``, as ``RingComm.shift``) -- in the half layout, the partner's whole
+        tensor."""
+        mine = mine.contiguous()
+        theirs = torch.empty_like(mine)
+        _cross_halves(self, mine, theirs, 1)
+        return theirs
+
+    def share(self, make, like: Tuple[tuple, torch.dtype, torch.device], chunks: int = 1) -> torch.Tensor:
+        """What ``make()`` returns for this rank's frames ([chunks * n_local, ...], ``(chunk, frame)``-major).  A rank
+        holding both CFG halves calls it.  In the half layouts it is computed once, on the ranks of half 0, each of
+        which sends every peer the rows of the frames they share; a half-1 rank receives its rows into a tensor of
+        ``like = (shape, dtype, device)`` without calling ``make``.  For everything drawn from an unseeded generator or
+        computed by a network outside this library, whose bits could differ between two devices."""
+        if not self.split_halves:
+            return make()
+        if self.half == 0:
+            out = make().contiguous()
+            _cross_halves(self, out, None, chunks)
+        else:
+            shape, dtype, device = like
+            out = torch.empty(shape, dtype=dtype, device=device)
+            _cross_halves(self, None, out, chunks)
+        return out
+
+    def gather_frames(self, t: torch.Tensor, chunks: int = 1) -> torch.Tensor:
+        """the whole ``(chunk, frame)``-major batch from every rank's block ``t`` of the exchange group
+        (``all_gather_frames``); ``t`` itself on one rank"""
+        if self.world == 1:
+            return t
+        return all_gather_frames(t, self.n_frames, self.world, chunks, self.group)
+
+    def ring(self) -> Optional["RingComm"]:
+        """the neighbour exchange of the frame ring: over the exchange group; None on one rank"""
+        return _comm(self.world, self.rank, self.group)
+
+    def trace_comm(self) -> Optional["RingComm"]:
+        """the communicator of every rank of the shard (loss sums over the batch); None on one rank"""
+        return _comm(*unpack(self.shard))
+
     def __repr__(self):
         return (f"ShardLayout(n_frames={self.n_frames}, halves={self.halves}, frames=[{self.lo}, {self.hi}), "
                 f"world={self.world}, rank={self.rank}, peers={self.peers})")
+
+
+def unpack(shard) -> Tuple[int, int, object]:
+    """(world, rank, group) of a ``shard=(world, rank[, group])`` tuple or ``Box``"""
+    return int(shard[0]), int(shard[1]), (shard[2] if len(shard) > 2 else None)
+
+
+def _comm(world: int, rank: int, group):
+    """the ``RingComm`` of ``group``, or the communicator injected in its place (tests: ranks as threads, an object
+    with ``shift``); None for one rank"""
+    if world == 1:
+        return None
+    return group if hasattr(group, "shift") else RingComm(world, rank, group)
 
 
 _HALF_GROUPS: dict = {}
@@ -191,9 +270,10 @@ def active_group(world: int, rank: int, group, active: int):
     return sub
 
 
-def shard_layout(n_frames: int, shard) -> Optional[ShardLayout]:
+def shard_layout(n_frames: int, shard) -> ShardLayout:
     """The partition of a keyframe batch of ``n_frames`` frames (2N samples: an unconditional and a text half) over
-    ``shard=(world, rank[, group])``; None for ``shard=None``.  Chosen by shape alone:
+    ``shard=(world, rank[, group])``; for ``shard=None`` the one-rank layout, which equals that of ``(1, 0, None)``.
+    A ``ShardLayout`` comes back as it is.  Chosen by shape alone:
 
     * N >= G: the frame layout -- rank r holds both halves of frames ``frame_range(N, G, r)``, the exchanges run on
       ``group``.
@@ -207,11 +287,10 @@ def shard_layout(n_frames: int, shard) -> Optional[ShardLayout]:
       * G > 2N: the first 2N ranks run the batch in the half layout, on their own process group (``active_group``);
         the others get an idle layout and take part in nothing."""
     if shard is None:
-        return None
+        shard = (1, 0, None)
     if isinstance(shard, ShardLayout):
         return shard
-    world, rank = int(shard[0]), int(shard[1])
-    group = shard[2] if len(shard) > 2 else None
+    world, rank, group = unpack(shard)
     box = isinstance(shard, Box)
     if box and world > 2 * n_frames:
         active = 2 * n_frames
@@ -243,11 +322,26 @@ def shard_layout(n_frames: int, shard) -> Optional[ShardLayout]:
     return ShardLayout(n_frames, (h, h + 1), lo, hi, sizes[h], r, sub, partner, shard, peers)
 
 
-def layout_group(layout: Optional[ShardLayout]):
-    """(world, rank, group) of the exchanges of ``layout``, as ``shard`` takes them; None when nothing is exchanged"""
-    if layout is None or layout.world == 1:
-        return None
-    return (layout.world, layout.rank, layout.group)
+def batch_layout(shard, flows, local: torch.Tensor, cfg_chunks: int, missing: str, count: bool = False) -> ShardLayout:
+    """``shard`` (None, a tuple, a ``Box`` or a ``ShardLayout``) resolved for a call that holds this rank's rows
+    ``local`` (``cfg_chunks`` CFG chunks of its frames) of a batch whose flows are ``flows`` (the whole batch's, or
+    None).  On one rank the batch is ``local``; otherwise its frame count is that of ``flows``.  Without flows a Box
+    raises ValueError(``missing``); a tuple sums the rows of the shard's ranks (one all-reduce) with ``count``, and
+    otherwise, having nothing to exchange without flows, runs as the one-rank layout of its own rows."""
+    if isinstance(shard, ShardLayout):
+        return shard
+    if shard is None or unpack(shard)[0] == 1:
+        return shard_layout(local.shape[0] // cfg_chunks, shard)
+    if flows is not None:
+        return shard_layout(int(flows[0].shape[0]), shard)
+    if isinstance(shard, Box):
+        raise ValueError(missing)
+    if not count:
+        return shard_layout(local.shape[0] // cfg_chunks, None)
+    # every (chunk, frame) sample is held once in either layout: the batch has (all rows) / chunks frames
+    rows = torch.full((1,), local.shape[0], dtype=torch.int64, device=local.device)
+    _comm(*unpack(shard)).all_reduce_sum(rows)
+    return shard_layout(int(rows.item()) // cfg_chunks, shard)
 
 
 def send_recv(sends, recvs, group=None) -> None:
@@ -288,35 +382,10 @@ def _cross_halves(layout: ShardLayout, send: Optional[torch.Tensor], recv: Optio
             buf = dst if dst.is_contiguous() else torch.empty(dst.shape, dtype=dst.dtype, device=dst.device)
             recvs.append((buf, peer))
             copies.append((dst, buf))
-    send_recv(sends, recvs, layout.shard[2] if len(layout.shard) > 2 else None)
+    send_recv(sends, recvs, unpack(layout.shard)[2])
     for dst, buf in copies:
         if buf is not dst:
             dst.copy_(buf)
-
-
-def partner_swap(layout: ShardLayout, mine: torch.Tensor) -> torch.Tensor:
-    """The other CFG half's rows of this rank's frames, shaped as ``mine`` ([n_local, ...]): one batched send / receive
-    with every peer (``send_recv``, as ``RingComm.shift``) -- in the half layout, the partner's whole tensor."""
-    mine = mine.contiguous()
-    theirs = torch.empty_like(mine)
-    _cross_halves(layout, mine, theirs, 1)
-    return theirs
-
-
-def partner_share(layout: ShardLayout, make, like: Tuple[tuple, torch.dtype, torch.device], chunks: int = 1) -> torch.Tensor:
-    """What ``make()`` returns for this rank's frames ([chunks * n_local, ...], ``(chunk, frame)``-major), computed once
-    on the ranks of half 0, each of which sends every peer the rows of the frames they share; a half-1 rank receives
-    its rows into a tensor of ``like = (shape, dtype, device)`` without calling ``make``.  Used for everything drawn
-    from an unseeded generator or computed by a network outside this library, whose bits could differ between two
-    devices."""
-    if layout.half == 0:
-        out = make().contiguous()
-        _cross_halves(layout, out, None, chunks)
-    else:
-        shape, dtype, device = like
-        out = torch.empty(shape, dtype=dtype, device=device)
-        _cross_halves(layout, None, out, chunks)
-    return out
 
 
 def chunk_frames(t: Optional[torch.Tensor], chunks: int, n_frames: int, lo: int, hi: int) -> Optional[torch.Tensor]:

@@ -135,20 +135,14 @@ def warp_tensor(sample, flows, occs, saliency, unet_chunk_size, shard=None):
     second all-to-all brings the frames back (SURVEY 8e, "sequential pieces").  When the channels do not split over the
     ranks (a decoded image has 3: background smoothing, src/pipe_FRESCO.py:46) every rank all-gathers the frames instead,
     runs the chain on the whole batch and keeps its own frames."""
-    layout = None
-    if shard is not None:
-        from .dist import shard_layout
-        layout = shard_layout(flows[0].shape[0], shard)
-        if layout.idle:
-            return sample                                       # an idle rank of a dist.Box holds no frame
-        if layout.world == 1 and not layout.split_halves:
-            layout = None                                       # one rank: the unsharded call
-    world = 1 if layout is None else layout.world
-    if layout is not None and layout.split_halves:
-        # one CFG half (or, in background smoothing, the decoded frames on the ranks of half 0): one chunk, the
-        # exchanges within the ranks of the half
-        unet_chunk_size = 1
-    n = sample.shape[0] // unet_chunk_size if layout is None else flows[0].shape[0]
+    from .dist import shard_layout
+    layout = shard_layout(flows[0].shape[0], shard)
+    if layout.idle:
+        return sample                                           # an idle rank of a dist.Box holds no frame
+    # a rank holding one CFG half (or, in background smoothing, the decoded frames on the ranks of half 0) holds one
+    # chunk, and the exchanges run within the ranks of its half
+    chunks = min(unet_chunk_size, layout.halves[1] - layout.halves[0])
+    world, n = layout.world, layout.n_frames
     h, w = sample.shape[2], sample.shape[3]
 
     bwd_flow, fwd_flow_last, blend = chain_operands(flows, occs, saliency, n, h, w)
@@ -164,23 +158,19 @@ def warp_tensor(sample, flows, occs, saliency, unet_chunk_size, shard=None):
             return t.float()
         return t
 
-    if world == 1:
-        if layout is not None and sample.shape[0] != n:
-            raise ValueError(f"warp_tensor: one CFG half of {n} frames needs {n} planes, got {sample.shape[0]}")
-        return chain(chain_input(sample.contiguous()), unet_chunk_size).to(sample.dtype)
-    import torch.distributed as dist
-    from .dist import all_gather_frames, block_sizes
-    group, rank = layout.group, layout.rank
-    chunks, C = unet_chunk_size, sample.shape[1]
     lo, hi = layout.lo, layout.hi
-    n_local = hi - lo
+    n_local, C = hi - lo, sample.shape[1]
     if sample.shape[0] != chunks * n_local:
-        raise ValueError(f"warp_tensor: rank {rank} of {world} owns frames [{lo}, {hi}) of {n}, "
+        raise ValueError(f"warp_tensor: rank {layout.rank} of {world} owns frames [{lo}, {hi}) of {n}, "
                          f"so sample needs {chunks * n_local} planes, got {sample.shape[0]}")
+    if world == 1:
+        return chain(chain_input(sample.contiguous()), chunks).to(sample.dtype)
+    import torch.distributed as dist
+    from .dist import block_sizes
     if C % world != 0:
         # gather path: the frames travel in the dtype of ``sample`` (fp16 VAE output: 1.5 MB per 512^2 frame), the chain
         # runs on exactly the batch the unsharded call sees
-        full = all_gather_frames(sample, n, world, chunks, group)                     # [chunk, frame, C, h, w]
+        full = layout.gather_frames(sample, chunks)                                   # [chunk, frame, C, h, w]
         fused = chain(chain_input(full), chunks).view(chunks, n, C, h, w)
         return fused[:, lo:hi].reshape(chunks * n_local, C, h, w).to(sample.dtype)
     x = chain_input(sample.contiguous())
@@ -189,11 +179,11 @@ def warp_tensor(sample, flows, occs, saliency, unet_chunk_size, shard=None):
     send = x.view(chunks, n_local, world, cg, h * w).permute(2, 1, 0, 3, 4).contiguous()      # [dest, frame, chunk, cg, hw]
     send = send.view(world * n_local, chunks * cg * h * w)
     recv = torch.empty(n, chunks * cg * h * w, dtype=x.dtype, device=x.device)
-    dist.all_to_all_single(recv, send, frames, [n_local] * world, group=group)   # [source rank = frame block, frame, ...]
+    dist.all_to_all_single(recv, send, frames, [n_local] * world, group=layout.group)   # [source rank = frame block, frame, ...]
     planes = recv.view(n, chunks * cg, h, w)                    # all N frames x my channel slice of both chunks
     fused = chain(planes, 1)
     back = torch.empty_like(send)
-    dist.all_to_all_single(back, fused.view(n, -1), [n_local] * world, frames, group=group)   # [source = channel block, ...]
+    dist.all_to_all_single(back, fused.view(n, -1), [n_local] * world, frames, group=layout.group)   # [source = channel block, ...]
     out = back.view(world, n_local, chunks, cg, h * w).permute(2, 1, 0, 3, 4).reshape(chunks * n_local, C, h, w)
     return out.contiguous().to(sample.dtype)
 

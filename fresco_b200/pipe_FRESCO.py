@@ -22,7 +22,7 @@ from typing import List, Optional
 import torch
 
 from . import ops
-from .dist import Box, layout_group, partner_share, partner_swap, shard_layout
+from .dist import ShardLayout, batch_layout, shard_layout
 from .flow_utils import warp_tensor
 
 
@@ -58,35 +58,23 @@ def step(pipe, model_output, timestep, sample, generator, repeat_noise=False, vi
     block, and the smoothing round trip runs on the ranks of half 0, which send its rows to their peers.  On an idle
     rank of a ``dist.Box`` it returns ``(sample, sample)`` at once.  A ``dist.Box`` itself takes the frame count from
     ``flows``; without them, pass its layout (``dist.shard_layout(N, box)``), as ``inference`` does."""
-    if isinstance(shard, Box):
-        if flows is None:
-            raise ValueError("step(shard=Box(...)) without flows does not know the batch's frame count: pass "
-                             "dist.shard_layout(n_frames, box)")
-        shard = shard_layout(int(flows[0].shape[0]), shard)
-    if getattr(shard, "idle", False):
+    layout = batch_layout(shard, flows, sample, 1, "step(shard=Box(...)) without flows does not know the batch's frame "
+                                                   "count: pass dist.shard_layout(n_frames, box)")
+    if layout.idle:
         return (sample, sample)
     alpha_prod_t, c_x0, c_xt, sigma = _step_coefficients(pipe.scheduler, timestep)
     sample = sample.contiguous()
     do_cfg = guidance_scale is not None
-    layout = shard if hasattr(shard, "split_halves") and shard.split_halves else None
-    if layout is not None:
-        if not do_cfg:
-            raise ValueError("a batch sharded over the CFG halves needs guidance_scale")
-        mine = model_output.contiguous()
-        theirs = partner_swap(layout, mine)
-        model_output = torch.cat([mine, theirs] if layout.half == 0 else [theirs, mine])
+    model_output = layout.guided(model_output, do_cfg)
     pred_original_sample = ops.cfg_pred_x0(model_output.contiguous(), sample, guidance_scale if do_cfg else 0.0,
                                            alpha_prod_t, do_cfg=do_cfg)
     if saliency is not None and flows is not None and occs is not None:                        # :44-47
         def smooth():
             image = pipe.vae.decode(pred_original_sample / pipe.vae.config.scaling_factor).sample
-            image = warp_tensor(image, flows, occs, saliency, unet_chunk_size=1, shard=shard)
+            image = warp_tensor(image, flows, occs, saliency, unet_chunk_size=1, shard=layout)
             return (pipe.vae.config.scaling_factor * pipe.vae.encode(image).latent_dist.sample()).contiguous()
-        if layout is None:
-            pred_original_sample = smooth()
-        else:
-            pred_original_sample = partner_share(layout, smooth, (pred_original_sample.shape, pred_original_sample.dtype,
-                                                                  pred_original_sample.device))
+        pred_original_sample = layout.share(smooth, (pred_original_sample.shape, pred_original_sample.dtype,
+                                                     pred_original_sample.device))
     if noise is None:
         noise = torch.randn(sample.shape, generator=generator, device=sample.device, dtype=sample.dtype)
     pred_prev_sample = ops.ddpm_prev(pred_original_sample, sample, noise.contiguous(), c_x0, c_xt, sigma,
@@ -94,16 +82,15 @@ def step(pipe, model_output, timestep, sample, generator, repeat_noise=False, vi
     return (pred_prev_sample, pred_original_sample)
 
 
-def _gather_first_last(latents_local, n, lo, hi, shard):
-    """[x_0, x_{N-1}] of the batch (src/pipe_FRESCO.py:177,179) when the frames are spread over ranks"""
-    if shard is None:
+def _gather_first_last(latents_local, layout: ShardLayout):
+    """[x_0, x_{N-1}] of the batch (src/pipe_FRESCO.py:177,179), whose frames may be spread over the exchange group"""
+    if layout.world == 1:
         return latents_local[[0, len(latents_local) - 1]].detach().clone()
     import torch.distributed as dist
-    world, rank, group = shard[0], shard[1], (shard[2] if len(shard) > 2 else None)
     mine = torch.stack([latents_local[0], latents_local[-1]])                  # my first / last frame
-    allp = torch.empty((world,) + tuple(mine.shape), dtype=mine.dtype, device=mine.device)
-    dist.all_gather_into_tensor(allp.view(-1, *mine.shape[1:]), mine, group=group)
-    return torch.stack([allp[0, 0], allp[world - 1, 1]]).clone()
+    allp = torch.empty((layout.world,) + tuple(mine.shape), dtype=mine.dtype, device=mine.device)
+    dist.all_gather_into_tensor(allp.view(-1, *mine.shape[1:]), mine, group=layout.group)
+    return torch.stack([allp[0, 0], allp[layout.world - 1, 1]]).clone()
 
 
 @torch.no_grad()
@@ -123,15 +110,13 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
     noise_scheduler = pipe.scheduler
     B, C, H, W = imgs.shape
     layout = shard_layout(B, shard)
-    if layout is not None and layout.idle:
+    if layout.idle:
         f = getattr(pipe, "vae_scale_factor", 8)
         return torch.empty(0, pipe.unet.config.in_channels, H // f, W // f, dtype=prompt_embeds.dtype, device=device)
     generator = torch.Generator(device=device).manual_seed(seed)
-    lo, hi = (0, B) if layout is None else (layout.lo, layout.hi)
-    split = layout is not None and layout.split_halves
-    chunks = 2 if do_classifier_free_guidance else 1
-    if split:
-        layout.chunks(chunks)                                                   # the halves need both CFG halves
+    lo, hi = layout.lo, layout.hi
+    cfg_chunks = 2 if do_classifier_free_guidance else 1
+    chunks = layout.chunks(cfg_chunks)                                          # the halves need both CFG halves
     if hasattr(frescoProc, "set_batch_frames"):
         frescoProc.set_batch_frames(B)
     latents = pipe.prepare_latents(B, pipe.unet.config.in_channels, H, W, prompt_embeds.dtype, device, generator,
@@ -145,13 +130,11 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
         def encode():
             return pipe.vae.config.scaling_factor * pipe.vae.encode(imgs[lo:hi].to(pipe.unet.dtype)).latent_dist.sample()
         # partners must hold the same latents: the posterior sample is drawn once, on the half-0 rank
-        latent_x0 = partner_share(layout, encode, (latents[lo:hi].shape, getattr(pipe.vae, "dtype", pipe.unet.dtype),
-                                                   latents.device)) if split else encode()
+        latent_x0 = layout.share(encode, (latents[lo:hi].shape, getattr(pipe.vae, "dtype", pipe.unet.dtype),
+                                          latents.device))
         latents_init = noise_scheduler.add_noise(latent_x0, latents[lo:hi], timesteps[num_warmup_steps]).detach()
     n_local = hi - lo
-    pe = prompt_embeds if layout is None else layout.rows(prompt_embeds, chunks)    # (b f) layout: the frames held
-    gather = layout_group(layout)                                               # record_latents: within the half
-    sub_flows = sub_occs = sub_sal = None
+    pe = layout.rows(prompt_embeds, cfg_chunks)                                 # (b f) layout: the frames held
     latents = latents_init
     for i, t in enumerate(timesteps[num_warmup_steps:]):
         if i >= num_intraattn_steps:
@@ -164,17 +147,17 @@ def inference(pipe, controlnet, frescoProc, imgs, prompt_embeds, edges, timestep
                 for f in range(2):
                     if lo <= f < hi:
                         latents[f - lo] = rec[f]
-            first_last = _gather_first_last(latents, B, lo, hi, gather)
+            first_last = _gather_first_last(latents, layout)
             if i < len(record_latents):
                 record_latents[i] = first_last
             else:                                                                # idle in the first batch of a Box
                 record_latents.append(first_last)
         else:
-            record_latents += [_gather_first_last(latents, B, lo, hi, gather)]
+            record_latents += [_gather_first_last(latents, layout)]
         # one CFG half per rank in the half layout: its latents, prompt and edge rows only
-        latent_model_input = torch.cat([latents] * 2) if do_classifier_free_guidance and not split else latents
+        latent_model_input = torch.cat([latents] * chunks) if chunks > 1 else latents
         if use_controlnet:
-            e = edges if layout is None else layout.rows(edges, chunks)
+            e = layout.rows(edges, cfg_chunks)
             down_block_res_samples, mid_block_res_sample = controlnet(
                 latent_model_input, t, encoder_hidden_states=pe, controlnet_cond=e,
                 conditioning_scale=cond_scale[i + num_warmup_steps], guess_mode=False, return_dict=False)

@@ -5,23 +5,15 @@ denoise step with guidance and background smoothing; an idle rank returns empty 
 the ranks share one GPU (transfers staged through host memory); nccl: one GPU each, skipped on a box with fewer, and
 there one step is also captured in a CUDA graph and replayed."""
 import os
-import sys
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
+from dist_harness import ROOT, Ctrl, NoCollectives, StubPipe, fb, finish, gpu_layer, init, rows, run  # noqa: F401
+
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-
-from test_gpu_dist_uneven import _finish, _init, _run, fb  # noqa: E402,F401
-
-
-def _rows(N, lay, dev):
-    return torch.cat([torch.arange(h * N + lay.lo, h * N + lay.hi) for h in range(*lay.halves)]).to(dev)
 
 
 class _FrameVAE:
@@ -48,41 +40,6 @@ class _FrameVAE:
         return Out
 
 
-def _layer(N, lay, box, dev):
-    from fresco_b200 import diffusion_hacked as dh
-    from fresco_b200.dist import ShardedFRESCOAttention
-    from test_gpu_parity_r2 import _trajectory_case
-    L, heads, C = 1024, 8, 640
-    g = torch.Generator().manual_seed(N * 7 + L)
-    q, k, v, rq, rk = (torch.randn(2 * N, L, C, generator=g).half().to(dev) for _ in range(5))
-    mask = torch.rand(N, L, generator=g) > 0.6
-    mask[0] = True
-    fwd, tmask = _trajectory_case(N, L, seed=3)
-    paras = {"fwd_mappings": [fwd[:, None].to(dev)], "bwd_mappings": [torch.argsort(fwd, 1)[:, None].to(dev)],
-             "interattn_masks": [tmask[:, None].to(dev)]}
-    proc = dh.FRESCOAttnProcessor2_0(2, dh.AttentionControl(), shard=box)
-    proc.set_batch_frames(N)
-    chunks = proc._layout.chunks(2)
-    sel = _rows(N, lay, dev)
-    bad = []
-    for flags in range(8):
-        ctrl = dh.AttentionControl()
-        if flags & 2:
-            ctrl.stored_attn["decoder_attn"] = [q]
-            ctrl.enable_intraattn()
-        if flags & 4:
-            ctrl.enable_interattn(paras)
-        if flags & 1:
-            ctrl.enable_cfattn([mask.to(dev)])
-        full = ShardedFRESCOAttention(ctrl, 1, 0, 2)(q, k, v, heads, ref_q=rq, ref_k=rk)
-        mine = ShardedFRESCOAttention(ctrl, lay.world, lay.rank, chunks, lay.group)(
-            q[sel].contiguous(), k[sel].contiguous(), v[sel].contiguous(), heads, ref_q=rq[sel].contiguous(),
-            ref_k=rk[sel].contiguous())
-        if not torch.equal(mine, full[sel]):
-            bad.append("attention flags %d: max |d| = %g" % (flags, (mine.float() - full[sel].float()).abs().max().item()))
-    return bad
-
-
 def _optimize(N, lay, box, dev):
     from fresco_b200 import diffusion_hacked as dh
     from test_gpu_parity_r2 import _layer_case
@@ -95,7 +52,7 @@ def _optimize(N, lay, box, dev):
     target = dh.gram_targets([ref])[0]
     tr_full, tr_mine = dh.OptimizeTrace(), dh.OptimizeTrace()
     full = dh.optimize_feature(sample, flows, occs, correlation_matrix=[target], iters=6, trace=tr_full)
-    sel = _rows(N, lay, dev)
+    sel = rows(N, lay, dev)
     mine = dh.optimize_feature(sample[sel].contiguous(), flows, occs, iters=6, trace=tr_mine, shard=box,
                                correlation_matrix=[dh.GramTarget(target.yhat[sel].contiguous())])
     bad = []
@@ -109,10 +66,8 @@ def _optimize(N, lay, box, dev):
 
 def _step_case(N, dev):
     from fresco_b200.harness import synth
-    from test_dist_cpu import _StubPipe
     ac = torch.from_numpy(np.load(os.path.join(ROOT, "tests", "golden", "ddpm_step.npz"))["alphas_cumprod"])
-    pipe = _StubPipe(ac)
-    pipe.vae = _FrameVAE()
+    pipe = StubPipe(ac, _FrameVAE)
     g = torch.Generator().manual_seed(6)
     eps, x, noise = (torch.randn(n, 4, 32, 32, generator=g).to(dev) for n in (2 * N, N, N))
     flows, occs = synth.smooth_flows(N, 256, 256, dev, seed=7)
@@ -124,7 +79,7 @@ def _step(N, lay, box, dev, graph):
     from fresco_b200 import pipe_FRESCO as pf
     pipe, eps, x, noise, flows, occs, sal = _step_case(N, dev)
     lo, hi = lay.lo, lay.hi
-    mine_eps = eps[_rows(N, lay, dev)].contiguous()
+    mine_eps = eps[rows(N, lay, dev)].contiguous()
     bad = []
     for smooth in (False, True) if N > 1 else (False,):         # the warp chain needs two frames
         kw = dict(flows=flows, occs=occs, saliency=sal) if smooth else {}
@@ -156,24 +111,13 @@ def _step(N, lay, box, dev, graph):
 
 def _idle(N, box, dev):
     """an idle rank: every entry point returns at once, with every collective of torch.distributed failing on use"""
-    import torch.distributed as dist
     from fresco_b200 import diffusion_hacked as dh
     from fresco_b200 import flow_utils as fu
     from fresco_b200 import pipe_FRESCO as pf
-    from test_dist_cpu import _Ctrl
-    names = ("all_gather_into_tensor", "all_to_all_single", "all_reduce", "broadcast", "batch_isend_irecv",
-             "new_group", "split_group")
-    saved = {n: getattr(dist, n) for n in names}
-
-    def fail(name):
-        def f(*a, **k):
-            raise AssertionError("torch.distributed.%s on an idle rank" % name)
-        return f
     bad = []
     pipe, eps, x, noise, flows, occs, sal = _step_case(N, dev)
-    for n in names:
-        setattr(dist, n, fail(n))
-    try:
+    with NoCollectives(("all_gather_into_tensor", "all_to_all_single", "all_reduce", "broadcast", "batch_isend_irecv",
+                        "new_group", "split_group")):
         none = x[:0]
         if pf.step(pipe, none, 700, none, None, guidance_scale=7.5, flows=flows, occs=occs, saliency=sal,
                    shard=box)[0] is not none:
@@ -182,30 +126,27 @@ def _idle(N, box, dev):
             bad.append("warp_tensor")
         if dh.optimize_feature(none, flows, occs, [], shard=box) is not none:
             bad.append("optimize_feature")
-        out = pf.inference(pipe, None, _Ctrl, torch.rand(N, 3, 256, 256, device=dev), torch.randn(2 * N, 5, 8, device=dev),
+        out = pf.inference(pipe, None, Ctrl, torch.rand(N, 3, 256, 256, device=dev), torch.randn(2 * N, 5, 8, device=dev),
                            None, [700], num_warmup_steps=0, use_controlnet=False, record_latents=[], shard=box)
         if tuple(out.shape) != (0, 4, 32, 32):
             bad.append("inference returned %s" % (tuple(out.shape),))
-    finally:
-        for n, f in saved.items():
-            setattr(dist, n, f)
     return bad
 
 
 def _box_worker(rank, world, port, ret, backend, N):
-    dev = _init(rank, world, port, backend)
+    dev = init(rank, world, port, backend)
     from fresco_b200.dist import Box, shard_layout
     box = Box(world, rank)
     lay = shard_layout(N, box)            # under NCCL every rank of the Box takes part in splitting its groups once
     if lay.idle:
         bad = _idle(N, box, dev) if rank >= 2 * N else ["rank %d idle" % rank]
     else:
-        bad = _layer(N, lay, box, dev) + _step(N, lay, box, dev, graph=backend == "nccl")
+        bad = gpu_layer(N, lay, box, dev) + _step(N, lay, box, dev, graph=backend == "nccl")
         if N > 1:
             bad += _optimize(N, lay, box, dev)
     for b in bad:
         print("rank %d of %d (%s), N %d: %s" % (rank, world, backend, N, b), flush=True)
-    _finish(rank, not bad, ret, dev)
+    finish(rank, not bad, ret, dev)
 
 
 @pytest.mark.parametrize("backend", ["gloo", "nccl"])
@@ -216,4 +157,4 @@ def test_box_bit_identical(fb, N, world, backend):
     The FRESCO layer (all 8 guidance flag combinations), optimize_feature with the ring halo (N = 2) and a denoise step
     with guidance, with and without background smoothing, equal the one-GPU call bit for bit on every active rank; over
     NCCL a captured step replays to the same bits."""
-    _run(_box_worker, world, backend, N)
+    run(_box_worker, world, backend, N, gpus=world if backend == "nccl" else 0)

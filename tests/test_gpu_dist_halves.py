@@ -4,75 +4,27 @@ sharing one GPU over gloo (and one GPU each over NCCL when the box has enough), 
 threads in lock step, and one harness-UNet denoise step in processes sharing one GPU (and over NCCL), which matches
 to the round-off of the UNet body at another batch size (REL_TOL)."""
 import os
-import sys
 import threading
 
 import numpy as np
 import pytest
 import torch
 
+from dist_harness import ROOT, fb, finish, gpu_layer, gpu_warp, init, rows, run  # noqa: F401
+
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-
-from test_gpu_dist_uneven import _finish, _init, _run, fb  # noqa: E402,F401
-
-
-def _half_rows(N, lay, dev):
-    base = lay.half * N
-    return torch.arange(base + lay.lo, base + lay.hi, device=dev)
 
 
 # ------------------------------------------------------------------------------------------------ the FRESCO layer
 def _layer_worker(rank, world, port, ret, backend, N):
-    dev = _init(rank, world, port, backend)
-    from fresco_b200 import diffusion_hacked as dh
-    from fresco_b200 import flow_utils as fu
-    from fresco_b200.dist import ShardedFRESCOAttention, shard_layout
-    from oracle import fresco_oracle as O
-    from test_gpu_parity_r2 import _trajectory_case
-    lay = shard_layout(N, (world, rank, None))
-    ok = lay.split_halves
-    L, heads, C, chunks = 1024, 8, 640, 2
-    g = torch.Generator().manual_seed(N * 7 + L)
-    q, k, v, rq, rk = (torch.randn(chunks * N, L, C, generator=g).half().to(dev) for _ in range(5))
-    mask = torch.rand(N, L, generator=g) > 0.6
-    mask[0] = True
-    fwd, tmask = _trajectory_case(N, L, seed=3)
-    paras = {"fwd_mappings": [fwd[:, None].to(dev)], "bwd_mappings": [torch.argsort(fwd, 1)[:, None].to(dev)],
-             "interattn_masks": [tmask[:, None].to(dev)]}
-    sel = _half_rows(N, lay, dev)
-    for flags in range(8):
-        ctrl = dh.AttentionControl()
-        if flags & 2:
-            ctrl.stored_attn["decoder_attn"] = [q]
-            ctrl.enable_intraattn()
-        if flags & 4:
-            ctrl.enable_interattn(paras)
-        if flags & 1:
-            ctrl.enable_cfattn([mask.to(dev)])
-        full = ShardedFRESCOAttention(ctrl, 1, 0, chunks)(q, k, v, heads, ref_q=rq, ref_k=rk)
-        mine = ShardedFRESCOAttention(ctrl, lay.world, lay.rank, 1, lay.group)(
-            q[sel].contiguous(), k[sel].contiguous(), v[sel].contiguous(), heads, ref_q=rq[sel].contiguous(),
-            ref_k=rk[sel].contiguous())
-        if not torch.equal(mine, full[sel]):
-            print("rank %d: attention flags %d differs: max |d| = %g"
-                  % (rank, flags, (mine.float() - full[sel].float()).abs().max().item()), flush=True)
-            ok = False
-    # warp_tensor within the half: a decoder feature of one CFG half and a decoded 512^2 image batch
-    flows, occs = O.synth_flows(N, 512, 512, seed=5, mag=12.0)
-    flows, occs = [f.to(dev) for f in flows], [o.to(dev) for o in occs]
-    sal = torch.rand(N, 1, 512, 512, generator=torch.Generator().manual_seed(2)).to(dev)
-    for chunks, shape, dtype in ((2, (640, 64, 64), torch.float16), (1, (3, 512, 512), torch.float32)):
-        x = torch.randn((chunks * N,) + shape, generator=torch.Generator().manual_seed(3)).to(dtype).to(dev)
-        rows = _half_rows(N, lay, dev) if chunks == 2 else torch.arange(lay.lo, lay.hi, device=dev)
-        full = fu.warp_tensor(x, flows, occs, sal, chunks)
-        mine = fu.warp_tensor(x[rows].contiguous(), flows, occs, sal, chunks, shard=lay.shard)
-        if not torch.equal(mine, full[rows]):
-            print("rank %d: warp_tensor %s differs" % (rank, (chunks * N,) + shape), flush=True)
-            ok = False
-    _finish(rank, ok, ret, dev)
+    dev = init(rank, world, port, backend)
+    from fresco_b200.dist import shard_layout
+    shard = (world, rank, None)
+    lay = shard_layout(N, shard)
+    bad = ([] if lay.split_halves else ["layout %r" % lay]) + gpu_layer(N, lay, shard, dev) + gpu_warp(N, lay, shard, dev)
+    for b in bad:
+        print("rank %d: %s" % (rank, b), flush=True)
+    finish(rank, not bad, ret, dev)
 
 
 @pytest.mark.parametrize("backend", ["gloo", "nccl"])
@@ -80,7 +32,7 @@ def test_sharded_layer_half_layout_bit_identical(fb, backend):
     """ShardedFRESCOAttention (all guidance flags) and warp_tensor at N = 3 on 4 ranks: rank r holds CFG half r // 2 of
     frames frame_range(3, 2, r % 2); == unsharded, bit for bit.  gloo: the ranks share one GPU; nccl: one GPU each,
     skipped on a box with fewer than 4."""
-    _run(_layer_worker, 4, backend, 3)
+    run(_layer_worker, 4, backend, 3, gpus=4 if backend == "nccl" else 0)
 
 
 # ------------------------------------------------------------------------------------------------ optimize_feature
@@ -155,7 +107,7 @@ def test_optimize_feature_half_layout_bit_identical(fb, N, world, C, h):
         try:
             comm = ring.comm(rank)
             lay = shard_layout(N, (world, rank, comm))
-            sel = _half_rows(N, lay, "cuda")
+            sel = rows(N, lay, "cuda")
             tgt = dh.GramTarget(target.yhat[sel].contiguous())
             tr = dh.OptimizeTrace()
             outs[rank] = (sel, dh.optimize_feature(sample[sel].contiguous(), flows, occs, correlation_matrix=[tgt],
@@ -180,7 +132,7 @@ def test_optimize_feature_half_layout_bit_identical(fb, N, world, C, h):
 
 # ------------------------------------------------------------------------------------------------ one denoise step
 def _step_worker(rank, world, port, ret, backend, N):
-    dev = _init(rank, world, port, backend)
+    dev = init(rank, world, port, backend)
     from fresco_b200 import diffusion_hacked as dh
     from fresco_b200 import flow_utils as fu
     from fresco_b200 import pipe_FRESCO as pf
@@ -218,15 +170,14 @@ def _step_worker(rank, world, port, ret, backend, N):
         proc.controller.enable_controller(interattn_paras=paras, attn_mask=attn_mask)
         outs.append(pf.inference(pipe, None, proc, imgs, pe, None, [t], num_warmup_steps=0, use_controlnet=False, seed=3,
                                  record_latents=[], step_interattn_end=0, shard=shard))
-    from fresco_b200.dist import partner_swap
     lay = shard_layout(N, (world, rank, None))
     mine, want = outs[1].float(), outs[0][lay.lo:lay.hi].float()
-    same_as_partner = bool(torch.equal(partner_swap(lay, outs[1]), outs[1]))
+    same_as_partner = bool(torch.equal(lay.swap(outs[1]), outs[1]))
     err, scale = (mine - want).abs().max().item(), want.abs().max().item()
     print("rank %d: max |sharded - unsharded| = %g of max |x| %g, partner bit-identical %s"
           % (rank, err, scale, same_as_partner), flush=True)
     ok = lay.split_halves and same_as_partner and err <= REL_TOL * scale
-    _finish(rank, ok, ret, dev)
+    finish(rank, ok, ret, dev)
 
 
 # The harness UNet body is not batch-invariant on the GPU: cuBLAS / cuDNN pick other algorithms at batch n than at 2N
@@ -238,7 +189,7 @@ REL_TOL = 1e-2
 
 
 @pytest.mark.parametrize("backend", ["gloo", "nccl"])
-@pytest.mark.parametrize("N,world", [(3, 4), (5, 8)])
+@pytest.mark.parametrize("N,world", [(2, 4), (3, 4), (3, 6), (4, 6), (5, 8), (7, 8)])
 def test_harness_denoise_step_half_layout_bit_identical(fb, N, world, backend):
     """One denoise step of the harness UNet with every FRESCO flag on (intra-frame targets, cross-frame, spatial- and
     temporal-guided attention, apply_FRESCO_opt on all four decoder layers) in the half layout: the processor builds
@@ -247,4 +198,4 @@ def test_harness_denoise_step_half_layout_bit_identical(fb, N, world, backend):
     frames of the unsharded step to REL_TOL (the UNet body's batch-size round-off).
     gloo: the ranks share one GPU (point-to-point transfers staged through host memory); nccl: one GPU each, skipped
     on a box with fewer."""
-    _run(_step_worker, world, backend, N)
+    run(_step_worker, world, backend, N, gpus=world if backend == "nccl" else 0)

@@ -2,127 +2,28 @@
 rank's share must equal the unsharded call bit for bit.  Ranks are processes sharing one GPU over gloo (and one GPU
 each over NCCL when the box has enough), or threads in lock step for the ring-halo feature optimisation; plus the
 loss-scale entry points of the Gram kernels against the weight entry points."""
-import os
-import socket
-import sys
 import threading
 
 import numpy as np
 import pytest
 import torch
 
+from dist_harness import fb, finish, gpu_inference, gpu_layer, gpu_warp, init, rows, run  # noqa: F401
+
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-
-
-@pytest.fixture(scope="module")
-def fb():
-    if not torch.cuda.is_available():
-        pytest.skip("GPU tests need a CUDA device")
-    from fresco_b200 import _lib
-    _lib.lib()      # fails loudly if the extension is missing
-
-
-def _init(rank, world, port, backend):
-    """``backend`` "nccl": one GPU per rank; "gloo": every rank on GPU 0, the exchanges through host memory"""
-    import torch.distributed as dist
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dev = torch.device("cuda", rank if backend == "nccl" else 0)
-    torch.cuda.set_device(dev)
-    if backend == "nccl":
-        dist.init_process_group("nccl", rank=rank, world_size=world, device_id=dev)
-    else:
-        dist.init_process_group("gloo", rank=rank, world_size=world)
-    return dev
-
-
-def _finish(rank, ok, ret, dev):
-    import torch.distributed as dist
-    t = torch.tensor([1 if ok else 0], device=dev)
-    dist.all_reduce(t, op=dist.ReduceOp.MIN)
-    if rank == 0:
-        ret.put(int(t.item()))
-    dist.destroy_process_group()
-
-
-def _run(worker, world, backend, *args):
-    import torch.multiprocessing as mp
-    if backend == "nccl" and torch.cuda.device_count() < world:
-        pytest.skip("needs %d GPUs" % world)
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    ctx = mp.get_context("spawn")
-    ret = ctx.Queue()
-    procs = [ctx.Process(target=worker, args=(r, world, port, ret, backend) + args) for r in range(world)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(600)
-        assert p.exitcode == 0
-    assert ret.get(timeout=5) == 1
-
-
-def _rows(n, lo, hi, chunks, dev):
-    return torch.cat([torch.arange(c * n + lo, c * n + hi) for c in range(chunks)]).to(dev)
 
 
 # ------------------------------------------------------------------------------------------------ attention + warp_tensor
 def _layer_worker(rank, world, port, ret, backend, N):
-    dev = _init(rank, world, port, backend)
-    from fresco_b200 import diffusion_hacked as dh
-    from fresco_b200 import flow_utils as fu
-    from fresco_b200.dist import ShardedFRESCOAttention, frame_range
-    from oracle import fresco_oracle as O
-    from test_gpu_parity_r2 import _trajectory_case
-    lo, hi = frame_range(N, world, rank)
-    ok = True
-    # level-A FRESCO layer: [2N, 1024, 640], 8 heads (d = 80); 1024 trajectories do not split evenly over 3 ranks
-    L, heads, C, chunks = 1024, 8, 640, 2
-    g = torch.Generator().manual_seed(N * 7 + L)
-    q, k, v, rq, rk = (torch.randn(chunks * N, L, C, generator=g).half().to(dev) for _ in range(5))
-    mask = torch.rand(N, L, generator=g) > 0.6
-    mask[0] = True
-    fwd, tmask = _trajectory_case(N, L, seed=3)
-    paras = {"fwd_mappings": [fwd[:, None].to(dev)], "bwd_mappings": [torch.argsort(fwd, 1)[:, None].to(dev)],
-             "interattn_masks": [tmask[:, None].to(dev)]}
-    sel = _rows(N, lo, hi, chunks, dev)
-    for flags in range(8):
-        ctrl = dh.AttentionControl()
-        if flags & 2:
-            ctrl.stored_attn["decoder_attn"] = [q]
-            ctrl.enable_intraattn()
-        if flags & 4:
-            ctrl.enable_interattn(paras)
-        if flags & 1:
-            ctrl.enable_cfattn([mask.to(dev)])
-        full = ShardedFRESCOAttention(ctrl, 1, 0, chunks)(q, k, v, heads, ref_q=rq, ref_k=rk)
-        mine = ShardedFRESCOAttention(ctrl, world, rank, chunks)(q[sel].contiguous(), k[sel].contiguous(), v[sel].contiguous(),
-                                                                 heads, ref_q=rq[sel].contiguous(), ref_k=rk[sel].contiguous())
-        if not torch.equal(mine, full[sel]):
-            print("rank %d: attention flags %d differs: max |d| = %g"
-                  % (rank, flags, (mine.float() - full[sel].float()).abs().max().item()), flush=True)
-            ok = False
-    # warp_tensor: a level-B decoder feature (640 channels: re-shard by channel on 2 ranks, gather on 3) and a decoded
-    # 512^2 image batch (3 channels: gather path, dilation and per-step chain kernels)
-    flows, occs = O.synth_flows(N, 512, 512, seed=5, mag=12.0)
-    flows, occs = [f.to(dev) for f in flows], [o.to(dev) for o in occs]
-    sal = torch.rand(N, 1, 512, 512, generator=torch.Generator().manual_seed(2)).to(dev)
-    for chunks, shape, dtype in ((2, (640, 64, 64), torch.float16), (1, (3, 512, 512), torch.float32)):
-        x = torch.randn((chunks * N,) + shape, generator=torch.Generator().manual_seed(3)).to(dtype).to(dev)
-        sel = _rows(N, lo, hi, chunks, dev)
-        full = fu.warp_tensor(x, flows, occs, sal, chunks)
-        mine = fu.warp_tensor(x[sel].contiguous(), flows, occs, sal, chunks, shard=(world, rank, None))
-        if not torch.equal(mine, full[sel]):
-            print("rank %d: warp_tensor %s differs" % (rank, (chunks * N,) + shape), flush=True)
-            ok = False
-    _finish(rank, ok, ret, dev)
+    dev = init(rank, world, port, backend)
+    from fresco_b200.dist import shard_layout
+    # 1024 trajectories do not split evenly over 3 ranks; the 640 channels re-shard on 2 ranks, gather on 3
+    shard = (world, rank, None)
+    lay = shard_layout(N, shard)
+    bad = gpu_layer(N, lay, shard, dev) + gpu_warp(N, lay, shard, dev)
+    for b in bad:
+        print("rank %d: %s" % (rank, b), flush=True)
+    finish(rank, not bad, ret, dev)
 
 
 @pytest.mark.parametrize("backend", ["gloo", "nccl"])
@@ -130,46 +31,23 @@ def _layer_worker(rank, world, port, ret, backend, N):
 def test_sharded_layer_uneven_bit_identical(fb, N, world, backend):
     """ShardedFRESCOAttention (all guidance flags) and warp_tensor on uneven frame blocks == unsharded, bit for bit.
     gloo: the ranks share one GPU; nccl: one GPU per rank, skipped on a box with fewer."""
-    _run(_layer_worker, world, backend, N)
+    run(_layer_worker, world, backend, N, gpus=world if backend == "nccl" else 0)
 
 
 def _inference_worker(rank, world, port, ret, backend, N):
-    dev = _init(rank, world, port, backend)
-    from fresco_b200 import pipe_FRESCO as pf
-    from fresco_b200.dist import frame_range
-    from oracle import fresco_oracle as O
-    from test_dist_cpu import _Ctrl
-    from test_gpu_dist_batch import _GPUStubPipe
-    lo, hi = frame_range(N, world, rank)
-    res = 512
-    ac = torch.from_numpy(np.load(os.path.join(ROOT, "tests", "golden", "ddpm_step.npz"))["alphas_cumprod"])
-    g = torch.Generator().manual_seed(1)
-    imgs = (torch.rand(N, 3, res, res, generator=g) * 2 - 1).half().to(dev)
-    pe = torch.randn(2 * N, 5, 8, generator=g).half().to(dev)
-    flows, occs = O.synth_flows(N, res, res, seed=9, mag=12.0)
-    flows, occs = [f.to(dev) for f in flows], [o.to(dev) for o in occs]
-    sal = (torch.rand(N, 1, res, res, generator=g) > 0.4).float().to(dev)
-    timesteps = [950 - 50 * i for i in range(20)]
-    ok = True
-    rec_full, rec_sh = [], []
-    for propagation in (False, True):
-        kw = dict(num_warmup_steps=14, use_controlnet=False, seed=3, repeat_noise=True, bg_smoothing_steps=[16, 17],
-                  propagation_mode=propagation, flows=flows, occs=occs, saliency=sal)
-        full = pf.inference(_GPUStubPipe(ac, dev), None, _Ctrl, imgs, pe, None, timesteps, record_latents=rec_full, **kw)
-        mine = pf.inference(_GPUStubPipe(ac, dev), None, _Ctrl, imgs, pe, None, timesteps, record_latents=rec_sh,
-                            shard=(world, rank, None), **kw)
-        same = bool(torch.equal(mine, full[lo:hi])) and len(rec_full) == len(rec_sh)
-        same = same and all(bool(torch.equal(a, b)) for a, b in zip(rec_full, rec_sh))
-        if not same:
-            print("rank %d: sharded inference differs (propagation=%s)" % (rank, propagation), flush=True)
-        ok = ok and same
-    _finish(rank, ok, ret, dev)
+    dev = init(rank, world, port, backend)
+    from fresco_b200.dist import shard_layout
+    shard = (world, rank, None)
+    bad = gpu_inference(N, shard_layout(N, shard), shard, dev, repeats=(True,))
+    for b in bad:
+        print("rank %d: %s" % (rank, b), flush=True)
+    finish(rank, not bad, ret, dev)
 
 
 @pytest.mark.parametrize("backend", ["gloo", "nccl"])
 def test_sharded_inference_uneven_bit_identical(fb, backend):
     """inference with background smoothing at 512^2 on frame blocks of 3 and 2 == unsharded, bit for bit"""
-    _run(_inference_worker, 2, backend, 5)
+    run(_inference_worker, 2, backend, 5, gpus=2 if backend == "nccl" else 0)
 
 
 # ------------------------------------------------------------------------------------------------ optimize_feature
@@ -180,7 +58,7 @@ def test_optimize_feature_ring_halo_uneven_bit_identical(fb, N, C, h, world):
     a rank's share of the weight rounded to fp32 gives another Gram loss scale than the unsharded call; the second is
     an even split."""
     from fresco_b200 import diffusion_hacked as dh
-    from fresco_b200.dist import frame_range
+    from fresco_b200.dist import shard_layout
     from test_gpu_parity_r2 import _LockstepRing, _layer_case
     flows, occs, cs = _layer_case(N, C, h, seed=31 + h)
     flows = [f.cuda() for f in flows]
@@ -196,8 +74,7 @@ def test_optimize_feature_ring_halo_uneven_bit_identical(fb, N, C, h, world):
     def run(rank):
         ring.lock.acquire()
         try:
-            lo, hi = frame_range(N, world, rank)
-            sel = _rows(N, lo, hi, 2, "cuda")
+            sel = rows(N, shard_layout(N, (world, rank, None)), "cuda")
             tgt = dh.GramTarget(target.yhat[sel].contiguous())
             outs[rank] = (sel, dh.optimize_feature(sample[sel].contiguous(), flows, occs, correlation_matrix=[tgt], iters=6,
                                                    shard=(world, rank, ring.comm(rank))))
